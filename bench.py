@@ -40,6 +40,8 @@ import torch  # noqa: E402
 
 H_IMG, W_IMG, C_IMG = 1080, 1920, 3
 BYTES_PER_PIX = 24.0  # algorithmic: 3 channels x 4 B read + 3 x 4 B written per output pixel
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3, 700 W card): the roofline's denominator, never a measured figure
+DUMP_SAMPLE = 1 << 22  # elements kept of a dumped output larger than this (16 MB as float32)
 METRIC = "Mpix/s warp_perspective Bx3x1080x1920 fwd bilinear fp32"
 
 
@@ -48,7 +50,7 @@ def headline_config(B: int, world: int) -> dict:
     configuration (stated in its `cpu_baseline.sample`), the metric is per pixel."""
     return {"workload": f"warp_perspective fwd B={B}x3x1080x1920 per GPU, bilinear, zeros, align_corners=True (BASELINE.json configs[1])",
             "global_batch": B * world, "parallelism": f"batch-sharded x{world}, no data-path collective",
-            "l2": "inputs (6.37 GB/GPU) exceed the 126 MB L2; no explicit flush",
+            "l2": "inputs (6.37 GB/GPU) exceed the 50 MB L2; no explicit flush",
             "homographies": "corner quad jittered by 8*randn px (benchmarks/geometry/flagship.py recipe), seed 1000+rank"}
 
 
@@ -80,6 +82,22 @@ def make_homographies_hw(B: int, seed: int, Hh: int, Ww: int) -> torch.Tensor:
 
 def make_homographies(B: int, seed: int) -> torch.Tensor:
     return make_homographies_hw(B, seed, H_IMG, W_IMG)
+
+
+def dump_outputs(dirname, arrays: dict) -> None:
+    """``--dump-outputs``: what the timed path returned in its last step, one ``<name>.npy`` per array (float64 stays float64,
+    everything else becomes float32).  An array of more than DUMP_SAMPLE elements is stored as the elements at DUMP_SAMPLE
+    flat indices drawn from a fixed seed (sorted), so two builds run with the same arguments can be compared value for value."""
+    import numpy as np
+
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().flatten()
+        if t.numel() > DUMP_SAMPLE:
+            idx = torch.randint(0, t.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(0)).sort().values
+            t = t[idx.to(t.device)]
+        t = t.double() if t.dtype == torch.float64 else t.float()
+        np.save(os.path.join(dirname, name + ".npy"), t.cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------ clocks
@@ -472,6 +490,8 @@ def run_ours(args) -> None:
     total_ms = t0.elapsed_time(t1)
     kern_ms = [s.elapsed_time(e) for (_, s, e) in timed_events]
     checksum = float(out[0, :, ::97, ::89].sum())  # touch the result
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"out": out})
     del out
     if dist is not None:
         t = torch.tensor([total_ms], device=dev)
@@ -496,20 +516,9 @@ def run_ours(args) -> None:
             dist.destroy_process_group()
         return
 
-    peaks, peak_src = None, "fallback 6650 GB/s (B200_PROFILING.md)"
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        peak = float(peaks["hbm_gbs"])
-        peak_src = "measured MEASURED_PEAKS.json hbm_gbs (burst copy)"
-    except Exception:
-        peak = 6650.0
+    peak = HBM_PEAK_GBS
     k_ms = statistics.mean(kern_ms) if kern_ms else float("nan")
     achieved = BYTES_PER_PIX * B * H_IMG * W_IMG / (k_ms * 1e-3) / 1e9
-    traffic = None
-    try:  # per-launch DRAM bytes of the same kernel from the committed ncu capture, if any
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "warp_fwd_traffic.json"))).get("dram_bytes_per_launch")
-    except Exception:
-        pass
 
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
@@ -530,8 +539,8 @@ def run_ours(args) -> None:
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic",
         "config": headline_config(B, world), "kernel_variant": variant,
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                     "kernel_ms": k_ms, "kernel_launches_timed": len(kern_ms), "peak_source": peak_src,
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
+                     "kernel_ms": k_ms, "kernel_launches_timed": len(kern_ms), "peak_source": "H100 SXM data sheet",
                      "algorithmic_bytes_per_launch": BYTES_PER_PIX * B * H_IMG * W_IMG},
         "cpu_baseline": cpu,
         "e2e": ({"value": pix_step / (e2e_ms * 1e-3) / 1e6, "unit": "Mpix/s", "h2d_bytes_per_step": bytes_step,
@@ -561,11 +570,7 @@ def run_extra(args) -> None:
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     torch.cuda.set_device(dev)
     _lib.load()
-    peak = 6650.0
-    try:
-        peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        pass
+    peak = HBM_PEAK_GBS
     torch.manual_seed(1000)
     if args.workload == "blur":
         B = args.batch
@@ -606,12 +611,14 @@ def run_extra(args) -> None:
     with ClockSampler(dev.index or 0) as clk:
         t0.record()
         for _ in range(args.steps):
-            step()
+            res = step()
         t1.record()
         torch.cuda.synchronize(dev)
         timed_events, _ops.kernel_events = (_ops.kernel_events or []), None
         launches = _ops.launch_count - launches0
         clk.hold_load(step, lambda: torch.cuda.synchronize(dev))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"out": res} if torch.is_tensor(res) else {"grad_src": res[0], "grad_M": res[1]})
     ms = t0.elapsed_time(t1) / args.steps
     kern = [s.elapsed_time(e) for (tg, s, e) in timed_events if tg == tag]
     k_ms = statistics.mean(kern) if kern else None
@@ -810,7 +817,7 @@ def run_scatter_gather(args) -> None:
         barrier()
         return max_ms(t0.elapsed_time(t1) / steps)
 
-    steps, warmup = max(2, min(args.steps, 5)), max(2, min(args.warmup, 3))
+    steps, warmup = args.steps, args.warmup
 
     def sg_step():
         return sharded_apply(lambda s, m: K.warp_perspective(s, m, dsize), (src, M if rank == 0 else None), batch=Bg,
@@ -829,7 +836,7 @@ def run_scatter_gather(args) -> None:
         shard = torch.rand(b - a, C_IMG, H_IMG, W_IMG, device=dev)
     src = None
     Ms = M[a:b].contiguous()
-    res_ms = timed(lambda: K.warp_perspective(shard, Ms, dsize), max(args.steps, 5), max(args.warmup, 3))
+    res_ms = timed(lambda: K.warp_perspective(shard, Ms, dsize), steps, warmup)
     if rank == 0:
         pix = Bg * H_IMG * W_IMG
         moved = (Bg - (b - a)) * C_IMG * H_IMG * W_IMG * 4  # bytes leaving rank 0 in the scatter (= bytes arriving in the gather)
@@ -852,7 +859,8 @@ def run_scatter_gather(args) -> None:
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (--workload small ignores it: it times >= 1 s of back-to-back "
+                    "calls per op by wall clock, the reference's published method)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--batch", type=int, default=256, help="samples per GPU")
@@ -865,7 +873,14 @@ def main() -> None:
     ap.add_argument("--workload", choices=["warp", "blur", "warp_bwd", "ingest", "small", "scatter_gather"], default="warp",
                     help="warp = the headline (BASELINE.json configs[1]); blur / warp_bwd = configs[2] / configs[3]; ingest = the uint8 wire-format warp "
                          "(SURVEY 8f row 4, not a BASELINE config); single GPU")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the last timed step returned as DIR/<name>.npy (float32; an output of "
+                         "more than 4 Mi elements as a fixed seeded sample of 4 Mi of them); warp, blur, warp_bwd and ingest workloads")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl == "reference" or args.workload in ("small", "scatter_gather")):
+        ap.error("--dump-outputs applies to the warp, blur, warp_bwd and ingest workloads of --impl ours")
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "small":

@@ -1,5 +1,5 @@
 /*
- * kornia_b200 -- C ABI of the B200-native warp / filter engine.
+ * kornia_b200 -- C ABI of the H100-native (sm_90a) warp / filter engine.
  *
  * The reference (kornia 0.9.0rc1) has no FFI: its boundary for this path is a set of Python
  * functions that bottom out in ATen calls.  Each entry point below replaces one such ATen
@@ -121,8 +121,7 @@ int kb200_remap_backward(const void* gout, const void* src, const void* map_x, c
  * maps never exist.  lens (B,16) = fx, fy, cx, cy, k1, k2, p1, p2, k3, k4, k5, k6, s1, s2, s3, s4 (the tilt terms of
  * the 14-coefficient model must be zero); src and out (B,C,H,W).  fp32, C in {1,3}, W % 4 == 0: anything else returns
  * KB200_EUNSUPPORTED and the host builds the maps and calls kb200_remap_forward.  Forward only.
- * Status: written after the round-1 GPU budget was spent -- compiled for sm_100a, not yet run on hardware; the Python
- * layer only calls it when KB200_FUSED_UNDISTORT=1. */
+ * The Python layer calls it when KB200_FUSED_UNDISTORT=1 (the default). */
 int kb200_undistort_forward(const void* src, const void* lens, void* out, int B, int C, int H, int W, int dtype, void* stream);
 
 /* Warp straight from a decoder's interleaved uint8 output (SURVEY.md 8f row 4): image_to_tensor
@@ -133,9 +132,7 @@ int kb200_undistort_forward(const void* src, const void* lens, void* out, int B,
  * device); 2 divides, as torch's CPU backend does (one ulp apart for 126 of the 256 byte values).  Forward only (a uint8 image has no gradient).
  * Bilinear (any of the four paddings), C in {1,3,4}, W % 4 == 0 and a 4-byte aligned src run the
  * shared-memory tiled kernel (warp_u8_tiled.cuh); everything else, or KB200_U8_SIMPLE=1, the per-tap kernel (warp_u8.cuh);
- * the two agree bit for bit.
- * Status: written after the round-1 GPU budget was spent -- compiled for sm_100a, executed on the host emulator, not yet
- * run on hardware. */
+ * the two agree bit for bit. */
 int kb200_warp_u8hwc_forward(const void* src_u8, const void* m, const void* bx, const void* by, const void* fill, void* out,
                              int B, int C, int H, int W, int h, int w, int Bm, int projective, int interp, int pad,
                              int align_corners, int normalize, void* stream);
@@ -186,8 +183,7 @@ int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void
  * 1 B written per input element instead of 8 + 5).  x (B,C,H,W), kernel (Bk,5,5) as in kb200_filter2d_forward,
  * out (B,C,H/2,W/2).  fp32, H even, W % 4 == 0, constant / reflect / replicate: anything else returns
  * KB200_EUNSUPPORTED and the host composes kb200_filter2d_forward with the resampling.
- * Status: written after the round-1 GPU budget was spent -- compiled for sm_100a, not yet run on hardware; the Python
- * layer only calls it when KB200_FUSED_PYRDOWN=1. */
+ * The Python layer calls it when KB200_FUSED_PYRDOWN=1 (the default). */
 int kb200_pyrdown_forward(const void* x, const void* kernel, void* out, int B, int C, int H, int W, int Bk, int border,
                           int dtype, void* stream);
 

@@ -1,4 +1,4 @@
-"""kornia_b200 -- B200-native (sm_100a) drop-in for Kornia's warp / filter hot path.
+"""kornia_b200 -- H100-native (sm_90a) drop-in for Kornia's warp / filter hot path.
 
     kornia.geometry.transform.{warp_perspective, warp_affine, remap}
     kornia.filters.{filter2d, filter2d_separable, gaussian_blur2d}

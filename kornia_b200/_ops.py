@@ -36,8 +36,8 @@ launch_count = 0
 def _require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
-            f"kornia_b200: {what} lives on {t.device}; this engine is CUDA-only (sm_100a) and has no CPU path. "
-            "Move the tensors to a B200 (`.cuda()`)."
+            f"kornia_b200: {what} lives on {t.device}; this engine is CUDA-only (sm_90a) and has no CPU path. "
+            "Move the tensors to an H100 (`.cuda()`)."
         )
 
 

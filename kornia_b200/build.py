@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA shared library for sm_100a (nvcc cross-compiles without a GPU)."""
+"""In-tree build of the CUDA shared library for sm_90a (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -14,7 +14,7 @@ OUT = os.path.join(OUT_DIR, "libkornia_b200.so")
 NVCC_FLAGS = [
     "-Xfatbin", "-compress-all",
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler", "-fPIC",
 ]
@@ -94,7 +94,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for f in os.listdir(obj_dir):  # objects of sources that no longer exist must not be linked by a later glob or linger
         if f.endswith(".o") and f not in known:
             os.remove(os.path.join(obj_dir, f))
-    cmd = [nvcc, "-shared", "-Xfatbin", "-compress-all", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs
+    cmd = [nvcc, "-shared", "-Xfatbin", "-compress-all", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT] + objs
     proc = subprocess.run(cmd, capture_output=True, text=True)
     if proc.returncode != 0:
         raise RuntimeError("link failed:\n" + " ".join(cmd) + "\n" + proc.stdout + proc.stderr)

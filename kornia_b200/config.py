@@ -2,15 +2,15 @@
 
 Every switch is read from the environment ONCE -- ``KB200_<NAME>=0|1`` when the package (for the host-side ones) or the
 shared library (for the device-side ones, include/kornia_b200.h: kb200_set_option) is loaded -- and can be changed
-afterwards only through this module; nothing on the call path touches ``os.environ``.  The defaults are the kernels that
-measured fastest on a B200 among bit-identical candidates (profiles/r2_variants_B64.txt); the parity tests flip a switch
+afterwards only through this module; nothing on the call path touches ``os.environ``.  Each default names, beside the
+kernel in csrc/, the measurement behind it and the GPU it was taken on; the parity tests flip a switch
 to run a kernel against the one it stands in for.
 
 Device-side (forwarded to the C library): ``tma`` (TMA-tiled warp / remap / backward kernels; off = generic per-pixel
 kernels), ``tiled_filter`` (shared-memory filter kernels; off = generic), ``square_tiles`` (second forward tile shape for
-rotated samples), ``sep_vwalk`` (band-walking separable filter: -1 auto = 11 taps and more, 0 never, 1 whenever it
+rotated samples), ``sep_vwalk`` (band-walking separable filter: 0 never, the default; -1 from 11 taps up; 1 whenever it
 applies), ``tiled_gradient``, ``u8_tiled`` (staged-window uint8 ingest warp; off = per-tap kernel), ``bwd_stride1`` (tiled
-backward on stride-1 lanes; off = column-pair lanes), ``remap_piped`` (pipelined persistent remap kernel for 'zeros' / 'border';
+backward on stride-1 lanes; off = column-pair lanes), ``remap_piped`` (pipelined persistent remap kernel for 'zeros' / 'border', off by default;
 off = one CTA per tile; 2 = also under 'reflection', for measurements), ``dyn_sched`` (warp forward and backward: the last rounds of
 strips / every warp's work drawn at run time from a per-device ring of counters; off = dealt out in advance), ``dyn_chunk`` (tiles
 per chunk, 10), ``dyn_static`` (percent of the full rounds the forward kernel still deals out in advance, 85).

@@ -29,7 +29,9 @@ void set_error(const char* fmt, ...) {
 
 // ---------------------------------------------------------------- kernel-selection switches (common.cuh: enum Option)
 static const char* const OPTION_NAMES[OPT_COUNT] = {"tma", "tiled_filter", "square_tiles", "sep_vwalk", "tiled_gradient", "u8_tiled", "bwd_stride1", "remap_piped", "dyn_sched", "dyn_chunk", "dyn_static"};
-static const int OPTION_DEFAULTS[OPT_COUNT] = {1, 1, 1, -1, 1, 1, 1, 1, 1, 10, 85};
+// sep_vwalk 0 and remap_piped 0: on an H100 SXM (700 W) the band walk lost to the tiled blur at 5-13 taps and tied at 17
+// (tools/ab_blur.py, B=256), and the pipelined remap lost 6-14 % with per-sample maps and tied with a shared map (tools/ab_remap.py, B=64)
+static const int OPTION_DEFAULTS[OPT_COUNT] = {1, 1, 1, 0, 1, 1, 1, 0, 1, 10, 85};
 static int g_options[OPT_COUNT];
 static const bool g_options_ready = [] {  // once, when the library is loaded: KB200_<NAME>=<int> overrides the default
   for (int i = 0; i < OPT_COUNT; ++i) {

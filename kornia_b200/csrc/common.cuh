@@ -1,4 +1,4 @@
-// kornia_b200 -- shared device/host helpers (sm_100a only).
+// kornia_b200 -- shared device/host helpers (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -73,6 +73,11 @@ __device__ __forceinline__ void st_stream(double* p, double v) { __stcs(p, v); }
 
 __host__ __device__ __forceinline__ int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// two fp32 FMAs on a pair of columns, each rounded once (sm_90 has no packed fp32 FMA: two FFMA per pair)
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // ---------------------------------------------------------------- kernel-selection switches (capi.cu)
 // Which of the library's own kernels serves a request.  Every switch is read from the environment ONCE, when the library is
 // loaded (KB200_<NAME>=0|1), and can be changed afterwards through kb200_set_option (tests compare a tiled kernel with the
@@ -105,9 +110,8 @@ inline void attribute_applied_on_device(unsigned long long& mask, int dev) { __a
 
 // Work counters of the run-time work distribution: a ring of 1 024 counters per device, allocated once (128 KB, the library's only
 // device allocation), one slot per launch, zeroed on the launch's stream.  A slot comes round again after 1 024 launches; two
-// launches could only share one if the first were still running then.  (The first version took each counter from the default
-// memory pool with cudaMallocAsync / cudaFreeAsync around the launch: whole runs of the headline bench then landed at 0.85 of the
-// roofline among runs at 0.93, profiles/r2_ab_headline_dyn.txt.)
+// launches could only share one if the first were still running then.  (A counter taken from the default memory pool with
+// cudaMallocAsync / cudaFreeAsync around each launch made whole runs of the headline bench markedly slower than others.)
 inline int* take_work_counter(cudaStream_t st) {
   constexpr int SLOTS = 1024, STRIDE = 32;  // ints: one counter per 128-byte line
   static int* base[64] = {nullptr};

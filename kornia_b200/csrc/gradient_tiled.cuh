@@ -8,8 +8,7 @@
 // LDS.128 -- the L1-gather kernel it replaces re-reads every input row K times through L1 with tiny CTAs (measured
 // 50-66 % of the HBM roofline, DESIGN.md 4.5).  MAG fuses sobel's sqrt(gx^2 + gy^2 + eps) (sobel.py:158-167).
 //
-// Status: written after the round-1 GPU budget was spent; compiled for sm_100a, not yet run on hardware.  Dispatched
-// only when KB200_TILED_GRADIENT=1 (gradient.cu).
+// Selected by the tiled_gradient switch (gradient.cu).
 #pragma once
 #include "filter2d_tiled.cuh"
 #include "gradient.cuh"

@@ -5,10 +5,9 @@
 // 72 x 40 x C source box, everything else on the exact per-pixel path) -- bit-identical results -- with the dependent chain
 // of that kernel taken off the critical path.
 //
-// What round 2 measured on remap_tiled_kernel (profiles/r2_remap_B16_ncu_digest.txt): 55-60 % of the 32 B/pixel roofline,
-// long-scoreboard 11.7 warps per issue slot, 13 % of the stall samples on the mbarrier spin.  One CTA per tile there runs
+// remap_tiled_kernel stalls on long-scoreboard waits and on its mbarrier spin.  One CTA per tile there runs
 //     map loads (DRAM latency) -> bounding box -> CTA barrier -> box load (DRAM latency again) -> blend -> exit
-// and only the four co-resident CTAs of an SM overlap each other's waits: too few bytes in flight for 6.5 TB/s.
+// and only the four co-resident CTAs of an SM overlap each other's waits: too few bytes in flight for HBM speed.
 // Here persistent CTAs (8 consumer warps + 1 producer warp, two per SM) walk strips of tiles and every load is a TMA load
 // issued tiles ahead of its use:
 //   * the map tiles (64 x 32 of map_x and of map_y) of tile t+2 are in flight while

@@ -41,8 +41,7 @@ static int launch_remap_piped(const CUtensorMap& msrc, const CUtensorMap& mmx, c
 int remap_piped_forward(const float* src, const float* map_x, const float* map_y, float* out, int B, int C, int H, int W, int h, int w,
                         int Bmap, int normalized, int pad, int align, cudaStream_t st) {
   if (!option(OPT_REMAP_PIPED)) return KB200_EUNSUPPORTED;
-  // measured (profiles/r2_ab_remap_B64.txt, three variants): under 'reflection' this kernel ends between 0.66x and 1.09x the
-  // one-CTA-per-tile kernel, which therefore keeps that mode
+  // under 'reflection' this kernel is not reliably faster than the one-CTA-per-tile kernel, which therefore keeps that mode
   if (pad == KB200_REFLECTION && option(OPT_REMAP_PIPED) < 2) return KB200_EUNSUPPORTED;  // remap_piped = 2: measure it anyway
   if ((w % 4) != 0 || ((reinterpret_cast<uintptr_t>(map_x) | reinterpret_cast<uintptr_t>(map_y)) & 15) != 0) return KB200_EUNSUPPORTED;
   if ((long long)B * ceil_div(h, 32) > 0x7fffffffll || (long long)B * C > 0x7fffffffll) return KB200_EUNSUPPORTED;

@@ -53,15 +53,14 @@ __device__ __forceinline__ float interior_reflection(float c) {
 // fmod = identity, span <= |c - lo| < 2 span has flips = 1 and fmod(a, span) = a - span EXACTLY (Sterbenz).  Anything further out
 // (or NaN) raises `far` and the caller sends the pixel to its exact path, where reflect_coord itself runs.  Bit-identical to
 // clip_coord(reflect_coord(...)) wherever `far` stays false (tools/hostemu checks it).
-// (Round 2, measured: with the general reflect_coord inlined as a third branch here, the 7 % border tiles of a 1080p warp cost
-//  3.5 x an interior tile and the pipelined remap ran at 34-48 % of its roofline -- profiles/r2_ab_remap_B64.txt.)
+// (With the general reflect_coord inlined as a third branch here, the border tiles of a 1080p warp cost several interior tiles.)
 template <typename T>
 __device__ __forceinline__ T reflect_clip_near_rt(T c, int size, bool align, bool& far) {
   using R = RN<T>;
   if (align) {
     // lo = 0, span = size - 1: c - 0 and e + 0 are the identity (e >= +0) and the reflected value already lies in [0, size - 1],
-    // so the clip is one too -- the general form below minus its four no-ops (16 -> 7 instructions per coordinate, which is what
-    // the 'reflection' remap was paying 32 times per pixel quad: profiles/r2_remap_piped_reflection_ncu_digest.txt)
+    // so the clip is one too -- the general form below minus its four no-ops (16 -> 7 instructions per coordinate, paid
+    // 32 times per pixel quad by the 'reflection' remap)
     if (size == 1) return T(0);  // a one-texel axis (uniform)
     const T span = T(size - 1);
     const T a = R::abs(c);
@@ -91,9 +90,8 @@ __device__ __forceinline__ T pad_coord(T c, int size, bool align) {
     c = clip_coord(c, size);
   } else if (PAD == KB200_REFLECTION) {
     // within one span of the image (all but pathological maps) the reflection is two subtractions and a select; only beyond that
-    // the general form with fmod / division runs.  Both agree bit for bit where the first applies.  (Measured, round 2: with the
-    // general form alone, the exact-path pixels of ONE badly fitting sample made its CTAs stragglers -- the 'reflection' warp took
-    // 765 us against 544 us for 'zeros' at B=64 with equal average SM time, profiles/r2_reflection_B64_straggler.txt.)
+    // the general form with fmod / division runs.  Both agree bit for bit where the first applies.  (With the
+    // general form alone, the exact-path pixels of ONE badly fitting sample make its CTAs stragglers.)
     bool far = false;
     const T near = reflect_clip_near_rt<T>(c, size, align, far);
     c = far ? clip_coord(align ? reflect_coord(c, 0, 2 * (size - 1)) : reflect_coord(c, -1, 2 * size - 1), size) : near;

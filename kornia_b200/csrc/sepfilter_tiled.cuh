@@ -11,8 +11,8 @@
 //   2. row pass: thread (q, r0) slides a K-tap window over 4 consecutive outputs of rows r0, r0+8, ...
 //      (aligned LDS.128 in, 4 x K FMAs, STS.128 out; all shared addresses are compile-time offsets)
 //      into a second shared tile;
-//   3. column pass: each thread owns 2 adjacent columns x 8 rows and accumulates with packed
-//      fma.rn.f32x2 (FFMA2) -- a column pair is a natural 64-bit register pair -- then streams out
+//   3. column pass: each thread owns 2 adjacent columns x 8 rows and accumulates two FFMAs per
+//      column pair (fma2_rn; a column pair is a natural 64-bit register pair), then streams out
 //      with 8-byte stores.
 // The taps stay in registers for a whole strip.  HBM traffic: 4 B read + 4 B written per element
 // (24 B per RGB pixel) plus halo re-reads that hit in L2; the eager reference moves >= 32 B per
@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(256, 3) sepfilter_tiled_kernel(const __grid_co
           const float2 v = m2[i * (TW / 2)];
 #pragma unroll
           for (int o = 0; o < RY; ++o) {
-            if (i - o >= 0 && i - o < K) acc[o] = __ffma2_rn(ky2[i - o], v, acc[o]);
+            if (i - o >= 0 && i - o < K) acc[o] = fma2_rn(ky2[i - o], v, acc[o]);
           }
         }
         if (LERP) {

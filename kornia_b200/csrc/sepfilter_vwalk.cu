@@ -23,10 +23,8 @@ static int launch_sep_vwalk(const CUtensorMap& map_main, const CUtensorMap& map_
 
 int sepfilter_vwalk_forward(const float* x, const float* kx, const float* ky, float* out, int B, int C, int H, int W, int Bkx, int kw,
                             int Bky, int kh, int border, int same, cudaStream_t st, const float* lerp_w) {
-  // Measured on B200, both kernels interleaved in one process at B=256x3x1080x1920 under sustained load
-  // (profiles/r2_ab_blur_B256.txt): the band walk wins from 11 taps up (11: 2.75 vs 2.83 ms, 13: 2.73 vs 2.95, 17: 2.80 vs 3.98) and
-  // loses below (5: 2.44 vs 2.22, 7: 2.49 vs 2.16, 9: 2.62 vs 2.36; the lerp epilogue of unsharp_mask 0.86 vs 0.69 ms at B=64), so
-  // that is the automatic rule.
+  // -1 = from 11 taps up, without the lerp epilogue of unsharp_mask.  Not the default: on an H100 SXM (700 W, B=256x3x1080x1920)
+  // the tiled kernel was faster at 5-13 taps (k=11: 5.20 vs 5.66 ms) and equal at 17 (tools/ab_blur.py, both kernels interleaved).
   const int sel = option(OPT_SEP_VWALK);
   if (sel == 0 || (sel < 0 && (kw < 11 || lerp_w)) || !option(OPT_TILED_FILTER)) return KB200_EUNSUPPORTED;
   if (!same || kw != kh || (kw & 1) == 0 || kw < 3 || kw > 17 || border == KB200_CIRCULAR) return KB200_EUNSUPPORTED;

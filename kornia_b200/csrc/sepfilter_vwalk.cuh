@@ -1,7 +1,7 @@
 // kornia_b200 -- separable K x K filter, one pass over HBM, walking DOWN column bands (fp32, 'same' padding).
 //
 // Same arithmetic as sepfilter_tiled_kernel (sepfilter_tiled.cuh: row pass with a register sliding window, column pass
-// on column pairs with packed FFMA2, ascending tap order -- bit-identical results) with a different walk.  There a CTA
+// on column pairs (two FFMAs per pair), ascending tap order -- bit-identical results) with a different walk.  There a CTA
 // moves left to right along a strip of 128 x 32 tiles and every tile row-filters its own 32 + K - 1 input rows: the
 // K - 1 halo rows are filtered twice (by the tile above and the tile below), and with 8 rows per sweep of the CTA the
 // 42 rows of the K = 11 blur take 6 sweeps, the last one three quarters idle -- the row pass costs 1.5x its useful work
@@ -16,8 +16,7 @@
 //     border is patched in the box, on the two edge bands only and only over the out-of-image columns.
 // Expected (not measured): ~18 % fewer issued instructions and 24 % less TMA / shared-memory fill traffic per tile.
 //
-// Status: written after the round-1 GPU budget was spent; compiled for sm_100a, not yet run on hardware.  Dispatched
-// only when KB200_SEP_VWALK=1 (sepfilter_vwalk.cu); tests/test_unverified_gpu.py compares it bit for bit with
+// Selected by the sep_vwalk switch (sepfilter_vwalk.cu); tests/test_variants_gpu.py compares it bit for bit with
 // sepfilter_tiled_kernel.
 #pragma once
 #include "sepfilter_tiled.cuh"
@@ -188,7 +187,7 @@ __global__ void __launch_bounds__(256, 3) sepfilter_vwalk_kernel(const __grid_co
           const float2 v = m2[i * (TW / 2)];
 #pragma unroll
           for (int o = 0; o < RY; ++o) {
-            if (i - o >= 0 && i - o < K) acc[o] = __ffma2_rn(ky2[i - o], v, acc[o]);
+            if (i - o >= 0 && i - o < K) acc[o] = fma2_rn(ky2[i - o], v, acc[o]);
           }
         }
         float* orow = p.out + (size_t)plane * p.H * p.W + (size_t)(y0 + yb * RY) * p.W + (size_t)x0 + 2 * cp;

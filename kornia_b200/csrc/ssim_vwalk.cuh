@@ -1,7 +1,7 @@
 // kornia_b200 -- SSIM index map in one pass, walking DOWN column bands with a TMA pipeline (fp32, odd K <= 11, reflect).
 //
 // Same arithmetic as ssim_tiled_kernel (ssim_tiled.cuh: products rounded on their own, five row sums with ascending
-// FMA taps, five column sums with packed FFMA2, the index with one rounding per reference op of
+// FMA taps, five column sums on column pairs (two FFMAs per pair), the index with one rounding per reference op of
 // kornia/metrics/ssim.py:92-139 -- bit-identical results), on the walk of sepfilter_vwalk_kernel.  The first version
 // gathers both boxes with scalar loads, synchronises, row-filters 32 + K - 1 rows, synchronises, column-filters: one
 // tile per CTA, nothing overlaps, measured 6.6 ms at B=64x3x1080x1920 (11 % of the HBM roofline, ~20 % of its FMA
@@ -13,9 +13,8 @@
 //   * the reflect border is a patch of the out-of-image box columns (edge bands only) and, vertically, a copy between
 //     row-filtered rows (first / last tile of a band only).
 //
-// Status: written after the round-1 GPU budget was spent; compiled for sm_100a, not yet run on hardware.  Dispatched
-// only when KB200_SSIM_VWALK=1 (ssim_vwalk.cu); tests/test_unverified_gpu.py compares it bit for bit with
-// ssim_tiled_kernel.
+// Launched by ssim_vwalk.cu; tests/test_variants_gpu.py checks it against the golden vectors, tools/hostemu bit for bit
+// against the scalar form.
 #pragma once
 #include "sepfilter_tiled.cuh"
 #include "filter_generic.cuh"
@@ -226,7 +225,7 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
             const float2 v = *reinterpret_cast<const float2*>(mid + (q * MH + rg * RY + i) * TW + 2 * cp);
 #pragma unroll
             for (int o = 0; o < RY; ++o) {
-              if (i - o >= 0 && i - o < K) acc[q][o] = __ffma2_rn(make_float2(k[i - o], k[i - o]), v, acc[q][o]);
+              if (i - o >= 0 && i - o < K) acc[q][o] = fma2_rn(make_float2(k[i - o], k[i - o]), v, acc[q][o]);
             }
           }
         }

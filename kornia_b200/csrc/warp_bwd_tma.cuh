@@ -7,14 +7,10 @@
 //   * d/dsrc: every warp owns a private 72x8xC accumulation strip in shared memory; taps are added with plain LDS/FADD/STS
 //     and the strip is added to global memory by ONE cp.reduce.async.bulk.tensor (TMA reduce-add, SASS UTMAREDG.3D.ADD) per
 //     warp and tile instead of twelve scattered atomics per pixel; out-of-image cells are clipped by the TMA unit.
-//     (Measured on B200: a TMA reduce with a negative box coordinate traps, so strip origins are clamped to >= 0.)
+//     (A TMA reduce with a negative box coordinate traps, so strip origins are clamped to >= 0.)
 //   * d/dM: taps come from a TMA-staged source window; the nine per-pixel partials accumulate in registers over a whole
 //     strip segment, then warp-shuffle -> one record per (CTA, segment, warp); a second kernel sums the records in a fixed
 //     order (deterministic, double accumulation).
-// History: round 1's first structure (one shared stage per CTA, CTA-wide mbarrier hand-off per tile) measured 1.90 ms at
-// B=128x3x720x1280 against 1.68 ms for warp_bwd_tma2 on the same B200 and was removed; so was a third structure (4-pixel
-// straight-line units on stride-1 lanes with rank-ordered rounds for lanes sharing a cell): its lane predicates compiled to
-// BSSY / BSYNC regions, 286 thread-instructions per pixel against 254, 2.15 ms (profiles/r2_bwd_tma3_ncu_digest.txt).
 #pragma once
 #include "warp_tma.cuh"
 

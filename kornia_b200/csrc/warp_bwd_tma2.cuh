@@ -5,8 +5,7 @@
 // shared-reciprocal IEEE division, strip adds with LDS/FADD/STS flushed by one TMA reduce-add per warp and tile,
 // d/dM partials in registers -> shuffle -> records -> fixed-order second stage), different synchronisation.
 //
-// What round 1 measured on warp_bwd_tma (profiles/r1_warp_bwd_tma_B32_ncu_digest.txt): issue-active 40 %, 12 % of all
-// stall samples on the consumers' mbarrier spin.  That kernel has ONE shared stage (the 72x40xC source box + the
+// warp_bwd_tma idles on the consumers' mbarrier spin.  That kernel has ONE shared stage (the 72x40xC source box + the
 // per-warp strip origins published by warp 0), so every tile ends with
 //     all warps -> `empty` -> warp 0 waits -> publishes + issues the box load -> box lands -> `full` -> all warps
 // and the CTA idles through that chain; the fast warps of a tile wait for the slowest.
@@ -19,8 +18,7 @@
 //   * no CTA-wide barrier or handshake inside the tile loop: 16 independent warps per SM hide each other's latency.
 // Shared memory: 8 x (window + strip) = 110.6 KB per CTA with both gradients -> still 2 CTAs/SM.
 //
-// Measured on B200 (round 2): bit-identical d/dsrc up to the order of the TMA reduce-adds; at B=128x3x720x1280 with both gradients
-// 1.71 ms on column-pair lanes, 1.62 ms on stride-1 lanes (STRIDE1, the default; round 1's shared-stage kernel: 1.90 ms).
+// d/dsrc is bit-identical to the column-pair lanes up to the order of the TMA reduce-adds; stride-1 lanes (STRIDE1) are the default.
 #pragma once
 #include <type_traits>
 
@@ -29,7 +27,7 @@
 namespace kb200 {
 
 // STRIDE1: lane <-> column (x0 + lane, x0 + 32 + lane) instead of column pairs (2 lane, 2 lane + 1).  Stride-2 lanes make every
-// strip / window access a 2-way bank conflict (half of the shared wavefronts in profiles/r2_first_bwd_ncu_digest.txt) but never
+// strip / window access a 2-way bank conflict but never
 // share a floor cell; stride-1 lanes are conflict-free but two neighbours fall into one cell wherever the map minifies.  The vote
 // stays warp-uniform: no duplicate in the instruction -> the un-predicated tap code; duplicates of multiplicity 2 -> two
 // predicated rounds (first-of-cell lanes, then second-of-cell lanes); deeper pile-ups -> the exact path.
@@ -37,8 +35,8 @@ namespace kb200 {
 // DYN: the work is not dealt out in advance.  The warps are independent pipelines already, so each WARP draws its next item -- one
 // 4-row slice of a chunk of tiles of a strip -- from a counter in global memory; the eight slices of a chunk are consecutive items.
 // No CTA-wide step is added.  The d/dM record of an item goes to row (chunk, slice), so the second stage sums the same partials in
-// a fixed order whatever warp produced them: still deterministic.  (Static deal, ncu at B=32: the slowest SM is active 23 % longer
-// than the average, profiles/r2_bwd_stride1_ncu_digest.txt.)
+// a fixed order whatever warp produced them: still deterministic.  (With a static deal the slowest SM is active
+// much longer than the average.)
 template <int NC, int PAD, bool PROJ, bool ALIGN, bool NEED_SRC, bool NEED_M, bool STRIDE1 = false, bool DYN = false>
 __global__ void __launch_bounds__(BWD_THREADS, 2) warp_bwd_tma2(const __grid_constant__ CUtensorMap tmap_srcwin,
                                                                 const __grid_constant__ CUtensorMap tmap_gsrc,

@@ -10,8 +10,7 @@
 // Algorithmic bytes per output pixel (C=3): 3 read + 12 written = 15, against 3+12 (ingest) + 12+12 (warp) = 39 for the
 // composition on the fp32 kernels of this library, and ~165 for the eager reference.
 //
-// First version: one thread per output pixel, taps through L1 (the structure of warp_fwd_generic).  Not yet run on
-// hardware (DESIGN.md section 9); the shared-memory staged form (byte boxes by TMA: rows of W*C bytes) is the next step.
+// First version: one thread per output pixel, taps through L1 (the structure of warp_fwd_generic); the shared-memory staged form (byte boxes by TMA: rows of W*C bytes) is the next step.
 #pragma once
 #include "warp_generic.cuh"
 

@@ -17,8 +17,7 @@
 // __syncthreads, so the CPU-side emulator (tools/hostemu) models everything this kernel does except speed.
 // Algorithmic bytes per RGB pixel: 3 read + 12 written.
 //
-// Status: written after the round-1 GPU budget was spent; compiled for sm_100a, executed on the emulator, not yet run on
-// hardware.  KB200_U8_SIMPLE=1 forces warp_fwd_u8hwc (tests compare the two bit for bit).
+// KB200_U8_SIMPLE=1 forces warp_fwd_u8hwc (tests compare the two bit for bit).
 #pragma once
 #include "remap_tiled.cuh"
 #include "warp_u8.cuh"

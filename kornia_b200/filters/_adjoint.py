@@ -1,5 +1,5 @@
-"""Input gradient of the one-pass separable filter without the four generic passes the autograd composition costs
-(DESIGN.md 6b / section 9).  Pure host logic over two primitives that are passed in, so that the band arithmetic can be
+"""Input gradient of the one-pass separable filter without the four generic passes the autograd composition costs.
+Pure host logic over two primitives that are passed in, so that the band arithmetic can be
 checked on CPU with the primitives swapped for torch ops (tests/test_filter_adjoint_host_logic.py):
 
   forward_constant(g, kx, ky)     'same' separable correlation of g with zero ('constant') border   -- the fast kernel

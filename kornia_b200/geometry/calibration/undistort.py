@@ -3,7 +3,7 @@ every output pixel is pushed through the lens model (``distort_points``) to find
 it, and the image is resampled there by ``remap`` -- the tiled TMA kernel of csrc/remap_tiled.cuh (bilinear,
 zeros, align_corners=True).  When no gradient is needed and the tilt coefficients are zero, the one-kernel form runs instead
 (kb200_undistort_forward: the lens model evaluated per pixel in registers, no maps, ~45 fewer elementwise passes):
-bit-identical to maps + remap on the same device and 17x faster on a B200 (profiles/r2_variants_B64.txt);
+bit-identical to maps + remap on the same device;
 ``config.set("fused_undistort", 0)`` selects the composition."""
 from __future__ import annotations
 
@@ -87,9 +87,7 @@ def undistort_image_from_uint8(image: torch.Tensor, K: torch.Tensor, dist: torch
     (kb200_undistort_u8hwc_forward: bytes staged and converted once per window, lens model per pixel, no maps) when no
     gradient is asked for, the tilt coefficients are zero, C is 1 or 3 and W % 4 == 0; otherwise the image is converted
     and ``undistort_image`` runs (differentiable w.r.t. ``K`` and ``dist``).  ``normalize`` as in
-    ``warp_perspective_from_uint8``: True / "device" (times 1/255, torch's CUDA ``x / 255.0``), "exact" (divided), False.
-
-    Status: the kernel has run on the host emulator only (DESIGN.md section 9)."""
+    ``warp_perspective_from_uint8``: True / "device" (times 1/255, torch's CUDA ``x / 255.0``), "exact" (divided), False."""
     from ..transform.ingest import _batched_hwc, _normalize_code
 
     image = _batched_hwc(image)

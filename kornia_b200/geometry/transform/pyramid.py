@@ -6,8 +6,8 @@ kernel of csrc/filter2d_tiled.cuh (border folded into the tile load, no ``F.pad`
 resampling step is ``torch.nn.functional.interpolate``, the third-party call the reference itself makes
 at pyramid.py:450-455,496-498 (the reference's own ``TODO: use kornia.geometry.resize``): 5 B/element of
 traffic next to the blur's 8.  At an exact factor of two (``align_corners=False``, no gradient) the resampling is a 2x2
-average and runs in the blur kernel's epilogue (kb200_pyrdown_forward): bit-identical to the composition and 2.2x faster on
-a B200 (profiles/r2_variants_B64.txt); ``config.set("fused_pyrdown", 0)`` selects the composition.  ``ScalePyramid`` (the SIFT octave builder) is a feature-
+average and runs in the blur kernel's epilogue (kb200_pyrdown_forward): bit-identical to the composition;
+``config.set("fused_pyrdown", 0)`` selects the composition.  ``ScalePyramid`` (the SIFT octave builder) is a feature-
 detection caller and stays out of scope."""
 from __future__ import annotations
 

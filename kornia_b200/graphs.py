@@ -1,11 +1,11 @@
-"""CUDA-graph replay of a launch-bound call (small images: a 32 x 3 x 256 x 256 warp is ~15 us of device work behind ~60 us of
-Python, dispatcher and launch cost).  ``GraphedCall(fn, *example_tensors)`` captures ``fn`` once on static buffers -- every kernel
+"""CUDA-graph replay of a launch-bound call (small images: a 32 x 3 x 256 x 256 warp is a few microseconds of device work behind
+several times as much Python, dispatcher and launch cost).  ``GraphedCall(fn, *example_tensors)`` captures ``fn`` once on static buffers -- every kernel
 of this library launches on the capturing stream and allocates nothing inside the C ABI, so prelude + warp + blur chains capture
 as they are -- and replays it per call: copy the inputs into the static buffers, one ``cudaGraphLaunch``, read the static output.
 Forward only, fixed shapes and dtypes (a new shape needs a new capture); the tensors returned are overwritten by the next call.
 
 The reference's answer to the same overhead is ``torch.compile`` (benchmarks/README.md:154: 96 k -> 232 k img/s); this is the
-B200-native one: streams and graphs instead of a tracing compiler."""
+H100-native one: streams and graphs instead of a tracing compiler."""
 from __future__ import annotations
 
 from typing import Callable, Sequence

@@ -1,10 +1,10 @@
 """Host-buffer pipeline: run a kernel of this library over a batch that lives in HOST memory.
 
-The kernels move 24 B per output pixel at ~5.8 TB/s; a batch that starts and ends in host memory is bound by the PCIe
-link instead (~55 GB/s per direction), so what matters end to end is that (a) the host-to-device copy of chunk i+1, the
-kernel of chunk i and the device-to-host copy of chunk i-1 overlap, and (b) the pinned host pages live on the NUMA node
-the GPU hangs off -- round 1 measured 46 GB/s per direction on one rank and 17.5 GB/s when eight unbound ranks shared the
-two sockets (SCALE_r01: e2e efficiency 0.38 at 8 GPUs).  This module is that pipeline as a library feature:
+The kernels move 24 B per output pixel at HBM speed (terabytes per second); a batch that starts and ends in host memory is
+bound by the PCIe link instead (tens of GB/s per direction), so what matters end to end is that (a) the host-to-device copy
+of chunk i+1, the kernel of chunk i and the device-to-host copy of chunk i-1 overlap, and (b) the pinned host pages live on
+the NUMA node the GPU hangs off: ranks whose buffers sit on the other socket share its interconnect and lose much of the
+PCIe bandwidth.  This module is that pipeline as a library feature:
 
 * :func:`bind_to_device_numa_node` pins the calling process (CPU affinity + preferred memory node) to the GPU's node;
 * :class:`HostPipeline` owns three streams, a ring of device staging buffers and the event choreography;

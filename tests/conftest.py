@@ -12,7 +12,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -29,11 +29,18 @@ def pytest_collection_modifyitems(config, items):
 
 
 class Golden:
-    """Reader for tests/golden/*.npz written by tests/golden/make_golden.py."""
+    """Reader for the shards tests/golden/<name>.<k>.npz written by tests/golden/make_golden.py (Bag.save)."""
 
     def __init__(self, name):
-        self._z = np.load(os.path.join(ROOT, "tests", "golden", name + ".npz"))
-        self.meta = json.loads(bytes(self._z["__meta__"]).decode())
+        self.meta, self._shard = {}, {}
+        k = 0
+        while os.path.exists(path := os.path.join(ROOT, "tests", "golden", f"{name}.{k}.npz")):
+            z = np.load(path)
+            meta = json.loads(bytes(z["__meta__"]).decode())
+            self.meta.update(meta)
+            self._shard.update(dict.fromkeys(meta, z))
+            k += 1
+        assert self.meta, f"no golden shards {name}.*.npz"
 
     def names(self, op=None):
         return [k for k, v in self.meta.items() if op is None or v["op"] == op]
@@ -41,9 +48,9 @@ class Golden:
     def case(self, name):
         import torch
 
-        m = self.meta[name]
-        ins = {k: torch.from_numpy(self._z[h].copy()) for k, h in m["inputs"].items()}
-        outs = {k: torch.from_numpy(self._z[h].copy()) for k, h in m["outputs"].items()}
+        m, z = self.meta[name], self._shard[name]
+        ins = {k: torch.from_numpy(z[h].copy()) for k, h in m["inputs"].items()}
+        outs = {k: torch.from_numpy(z[h].copy()) for k, h in m["outputs"].items()}
         return m["op"], dict(m["kwargs"]), ins, outs
 
 

@@ -10,10 +10,12 @@ never calls it: SURVEY.md section 8c).  Every case stores the exact inputs, the 
 (JSON) and the reference's CPU fp32 outputs (plus autograd gradients where marked), so the
 fixtures travel to the GPU box where /root/reference does not exist.
 
-Output: tests/golden/warp.npz, tests/golden/filter.npz (about 2.5 MB each; inputs are stored once, content-addressed).
+Output: tests/golden/warp.*.npz, tests/golden/filter.*.npz (shards under 1 MB; inputs are stored once per shard,
+content-addressed).
 """
 from __future__ import annotations
 
+import glob
 import hashlib
 import json
 import os
@@ -62,10 +64,31 @@ class Bag:
             "outputs": {k: self._put(v) for k, v in outputs.items()},
         }
 
+    SHARD_BYTES = 800_000  # uncompressed array bytes per shard: every stored file stays under 1 MB
+
     def save(self, path):
-        self.arrays["__meta__"] = np.frombuffer(json.dumps(self.meta).encode(), dtype=np.uint8)
-        np.savez_compressed(path, **self.arrays)
-        print(f"{path}: {len(self.meta)} cases, {os.path.getsize(path) / 1024:.0f} kB")
+        """``x.npz`` is written as shards ``x.0.npz``, ``x.1.npz``, ... of whole cases, each with the ``__meta__`` of its
+        cases (an input shared by cases of two shards is stored in both); tests/conftest.py:Golden reads them back as one."""
+        stem = path[: -len(".npz")]
+        for old in glob.glob(glob.escape(stem) + ".*.npz"):  # a save with fewer shards must not leave stale cases behind
+            os.remove(old)
+        shards, keys, size = [], None, 0
+        for name, m in self.meta.items():
+            need = set(m["inputs"].values()) | set(m["outputs"].values())
+            extra = sum(self.arrays[k].nbytes for k in need - (keys or set()))
+            if keys is None or (size + extra > self.SHARD_BYTES and shards[-1]):
+                shards.append({})
+                keys, size = set(), 0
+                extra = sum(self.arrays[k].nbytes for k in need)
+            shards[-1][name] = m
+            keys |= need
+            size += extra
+        for i, meta in enumerate(shards):
+            arrays = {k: self.arrays[k] for m in meta.values() for k in list(m["inputs"].values()) + list(m["outputs"].values())}
+            arrays["__meta__"] = np.frombuffer(json.dumps(meta).encode(), dtype=np.uint8)
+            np.savez_compressed(f"{stem}.{i}.npz", **arrays)
+        print(f"{stem}.*.npz: {len(self.meta)} cases in {len(shards)} shards of at most "
+              f"{max(os.path.getsize(f'{stem}.{i}.npz') for i in range(len(shards))) / 1024:.0f} kB")
 
 
 def smooth_image(B, C, H, W, gen):

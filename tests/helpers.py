@@ -1,5 +1,64 @@
 """Shared helpers for the parity tests: dispatch a golden case onto an implementation module."""
+import contextlib
+import os
+import sys
+
 import torch
+
+# The import graph of the kornia package that install() has to patch: the modules that define the hot-path functions, the
+# package re-exports, and the importers of kornia 0.9 (``from ... import warp_perspective``-style and ``from kornia import
+# metrics``).  Function bodies do not matter to install(); every defining module gets stand-ins of its names.
+_STANDIN_KORNIA = {
+    "__init__": "from . import filters, geometry, metrics, losses, augmentation",
+    "geometry/transform/imgwarp": "def warp_perspective(): pass\ndef warp_affine(): pass\ndef remap(): pass\ndef get_perspective_transform(): pass",
+    "filters/filter": "def filter2d(): pass\ndef filter2d_separable(): pass",
+    "filters/gaussian": "def gaussian_blur2d(): pass",
+    "filters/sobel": "def spatial_gradient(): pass\ndef sobel(): pass",
+    "filters/unsharp": "from .gaussian import gaussian_blur2d",
+    "filters/__init__": "from .filter import filter2d, filter2d_separable\nfrom .gaussian import gaussian_blur2d\n"
+                        "from .sobel import sobel, spatial_gradient\nfrom . import unsharp",
+    "metrics/ssim": "def ssim(): pass",
+    "metrics/__init__": "from .ssim import ssim",
+    "losses/ssim": "from kornia import metrics",
+    "losses/__init__": "from . import ssim",
+    "geometry/__init__": "from . import transform, calibration\nfrom .transform import warp_perspective, warp_affine, remap",
+    "geometry/transform/__init__": "from .imgwarp import warp_perspective, warp_affine, remap, get_perspective_transform\n"
+                                   "from . import affwarp, crop2d, pyramid",
+    "geometry/transform/affwarp": "from kornia.filters import gaussian_blur2d\nfrom .imgwarp import warp_affine",
+    "geometry/transform/crop2d": "from .imgwarp import get_perspective_transform, warp_affine, warp_perspective",
+    "geometry/transform/pyramid": "from kornia.filters import filter2d, gaussian_blur2d",
+    "geometry/calibration/__init__": "from . import undistort",
+    "geometry/calibration/undistort": "from kornia.geometry.transform import remap",
+    "augmentation/__init__": "from . import _2d",
+    "augmentation/_2d/__init__": "from . import geometric, intensity",
+    "augmentation/_2d/geometric/__init__": "from . import perspective",
+    "augmentation/_2d/geometric/perspective": "from kornia.geometry.transform import get_perspective_transform, warp_perspective",
+    "augmentation/_2d/intensity/__init__": "from . import gaussian_blur",
+    "augmentation/_2d/intensity/gaussian_blur": "from kornia.filters import gaussian_blur2d",
+}
+
+
+@contextlib.contextmanager
+def standin_kornia(tmp_dir):
+    """Import a stand-in ``kornia`` package (the import graph above, written under ``tmp_dir``); removed again on exit."""
+    for mod, src in _STANDIN_KORNIA.items():
+        path = os.path.join(tmp_dir, "kornia", mod + ".py")
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with open(path, "w") as f:
+            f.write(src + "\n")
+    saved = {k: v for k, v in sys.modules.items() if k == "kornia" or k.startswith("kornia.")}
+    for k in saved:
+        del sys.modules[k]
+    sys.path.insert(0, str(tmp_dir))
+    try:
+        import kornia
+
+        yield kornia
+    finally:
+        sys.path.remove(str(tmp_dir))
+        for k in [k for k in sys.modules if k == "kornia" or k.startswith("kornia.")]:
+            del sys.modules[k]
+        sys.modules.update(saved)
 
 
 def _tup(v):

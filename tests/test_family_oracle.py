@@ -10,7 +10,7 @@ import torch
 
 import kornia_b200 as K
 from conftest import golden
-from helpers import family_grads, rel_l2, run_family_case
+from helpers import family_grads, rel_l2, run_family_case, standin_kornia
 from oracle import kornia_restated as R
 
 FAM = golden("family")
@@ -144,16 +144,8 @@ def test_module_forms():
     assert KF.UnsharpMask((3, 3), (1.0, 1.0)).border_type == "reflect"
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/kornia"), reason="needs the reference checkout (build container only)")
-def test_install_rebinds_every_importer_of_the_reference():
-    import sys
-    import tempfile
-
-    stub = tempfile.mkdtemp(prefix="kornia_rs_stub_")
-    open(os.path.join(stub, "kornia_rs.py"), "w").close()
-    sys.path[:0] = [stub, "/root/reference"]
-    try:
-        import kornia
+def test_install_rebinds_every_importer_of_the_reference(tmp_path):
+    with standin_kornia(tmp_path) as kornia:
         import kornia.augmentation._2d.geometric.perspective as aug_persp
         import kornia.augmentation._2d.intensity.gaussian_blur as aug_blur
         import kornia.geometry.transform.affwarp as affwarp
@@ -179,9 +171,6 @@ def test_install_rebinds_every_importer_of_the_reference():
             K.uninstall()
         assert kornia.geometry.transform.warp_perspective is orig and aug_persp.warp_perspective is orig
         assert kornia.metrics.ssim is not K.metrics.ssim and callable(kornia.filters.sobel)
-    finally:
-        sys.path.remove(stub)
-        sys.path.remove("/root/reference")
 
 
 def test_fused_unsharp_request_host_logic():

@@ -1,6 +1,5 @@
-"""Kernel variants against the kernels they stand in for (kornia_b200.config switches).  Every kernel here first met a B200
-in round 2 (tools/r2_first_call.sh: 332 of these comparisons passed on the first run); the ones that measured faster are the
-defaults now, the rest were removed.  Each test flips a switch, runs both kernels on the same inputs and compares bit for bit
+"""Kernel variants against the kernels they stand in for (kornia_b200.config switches).  The ones that measured faster are the
+defaults.  Each test flips a switch, runs both kernels on the same inputs and compares bit for bit
 where the arithmetic is the same, and checks the golden vectors recorded from the reference."""
 import pytest
 import torch
@@ -147,7 +146,7 @@ def test_band_walk_ssim_bit_identical(window, shape):
 
 
 def test_band_walk_ssim_many_segments_and_golden():
-    a = torch.rand(40, 3, 200, 260, device=DEV)   # 120 planes x 5 bands = 600 bands > 296 CTAs: segments start inside bands
+    a = torch.rand(40, 3, 200, 260, device=DEV)   # 120 planes x 5 bands = 600 bands > the persistent grid (2 CTAs per SM): segments start inside bands
     b = a.flip(-1).contiguous()
     got = K.metrics.ssim(a, b, 11)
     assert torch.equal(got, K.metrics.ssim(a.clone().requires_grad_(True), b, 11).detach())

@@ -10,7 +10,7 @@ import torch
 
 import kornia_b200 as K
 from conftest import golden
-from helpers import family_grads, rel_l2, run_family_case
+from helpers import family_grads, rel_l2, run_family_case, standin_kornia
 from oracle import kornia_restated as R
 
 WID = golden("wider")
@@ -152,19 +152,10 @@ def test_tilt_projection_matches_oracle():
     assert KC.tilt_projection(torch.tensor(0.1), torch.tensor(0.2)).shape == (3, 3)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/kornia"), reason="needs the reference checkout (build container only)")
-def test_install_reaches_the_new_callers():
+def test_install_reaches_the_new_callers(tmp_path):
     """install() rebinds filter2d / gaussian_blur2d / remap inside the reference's pyramid, affwarp and undistort modules,
     so the reference's own pyrdown / resize(antialias) / undistort_image run on the CUDA kernels unmodified."""
-    import sys
-    import tempfile
-
-    stub = tempfile.mkdtemp(prefix="kornia_rs_stub_")
-    open(os.path.join(stub, "kornia_rs.py"), "w").close()
-    sys.path[:0] = [stub, "/root/reference"]
-    try:
-        import kornia
-
+    with standin_kornia(tmp_path) as kornia:
         pyr = import_module("kornia.geometry.transform.pyramid")
         aff = import_module("kornia.geometry.transform.affwarp")
         und = import_module("kornia.geometry.calibration.undistort")
@@ -174,9 +165,6 @@ def test_install_reaches_the_new_callers():
         finally:
             K.uninstall()
         assert pyr.filter2d is not K.filter2d
-    finally:
-        sys.path.remove(stub)
-        sys.path.remove("/root/reference")
 
 
 def test_lens_packing_and_kernel_op_order():

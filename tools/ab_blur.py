@@ -36,4 +36,4 @@ for k in (5, 7, 9, 11, 13, 17):
     K.config.reset()
     a, b = min(res[0]), min(res[1])
     gb = 24.0 * B * 1080 * 1920 / 1e6
-    print(f"k={k:2d} B={B}: {SWITCH}=0 {a:.3f} ms ({gb / a / 6568 * 100:.1f} %)  {SWITCH}=1 {b:.3f} ms ({gb / b / 6568 * 100:.1f} %)  all: {['%.3f' % v for v in res[0]]} {['%.3f' % v for v in res[1]]}", flush=True)
+    print(f"k={k:2d} B={B}: {SWITCH}=0 {a:.3f} ms ({gb / a / 3350 * 100:.1f} %)  {SWITCH}=1 {b:.3f} ms ({gb / b / 3350 * 100:.1f} %)  all: {['%.3f' % v for v in res[0]]} {['%.3f' % v for v in res[1]]}", flush=True)

@@ -39,4 +39,4 @@ for rep in range(4):
 gb = 24.0 * B * 1080 * 1920 / 1e6
 for v in (0, 1):
     a = min(res[v])
-    print(f"dyn_sched={v}: {a:.4f} ms / call ({gb / a / 6568 * 100:.1f} % of 6.57 TB/s)  all: {['%.4f' % r for r in res[v]]}", flush=True)
+    print(f"dyn_sched={v}: {a:.4f} ms / call ({gb / a / 3350 * 100:.1f} % of 3.35 TB/s)  all: {['%.4f' % r for r in res[v]]}", flush=True)

@@ -49,5 +49,5 @@ for pad in ("zeros", "border", "reflection"):
         a = min(ms for p, ms in rows if p == 0)
         b = min(ms for p, ms in rows if p == 1)
         gb = bpp * B * 1080 * 1920 / 1e6
-        print(f"{pad:10s} {name:24s} bit-identical={same}  per-tile {a:.3f} ms ({gb/a/6568*100:4.1f} %)  piped {b:.3f} ms ({gb/b/6568*100:4.1f} %)  x{a/b:.2f}   all: "
+        print(f"{pad:10s} {name:24s} bit-identical={same}  per-tile {a:.3f} ms ({gb/a/3350*100:4.1f} %)  piped {b:.3f} ms ({gb/b/3350*100:4.1f} %)  x{a/b:.2f}   all: "
               + " ".join(f"{p}:{ms:.3f}" for p, ms in rows), flush=True)

@@ -1,7 +1,7 @@
 """Timing of the filter / affine family (SURVEY.md 8f rows 2-3) at B x 3 x 1080 x 1920 fp32 on one GPU: this
 library vs the reference's torch composition (the oracle module, i.e. the same ATen calls the reference makes)
 on the same device.  CUDA events, 3 warm-ups, inputs (>= 1.6 GB) larger than L2.  Prints one line per op with the
-algorithmic bytes moved per second and the fraction of the measured HBM roofline (MEASURED_PEAKS.json)."""
+algorithmic bytes moved per second and the fraction of the HBM roofline (3.35 TB/s, H100 SXM data sheet)."""
 import json
 import os
 import sys
@@ -16,11 +16,7 @@ from oracle import kornia_restated as R  # noqa: E402
 dev = "cuda"
 B = int(os.environ.get("FAMILY_B", "64"))
 H, W = 1080, 1920
-peak = 6568.0
-try:
-    peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-except Exception:
-    pass
+peak = 3350.0
 x = torch.rand(B, 3, H, W, device=dev)
 elems = B * 3 * H * W
 

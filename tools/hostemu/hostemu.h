@@ -5,8 +5,8 @@
 //   tma::load_3d()         copies the box (zero fill outside the tensor) and completes bytes on the mbarrier -- at once in
 //                          EAGER mode, or only when no fiber can make progress in LAZY mode.  EAGER exposes a load that
 //                          lands on data still being read, LAZY exposes a read that does not wait for its load.
-// The emulator checks what the hardware would trap or hang on: 16-byte aligned innermost coordinate (measured to trap
-// on B200: tools/tma_probe.cu), 128-byte aligned destination, byte counts that match expect_tx, deadlocks.
+// The emulator checks what the hardware would trap or hang on: 16-byte aligned innermost coordinate (traps,
+// tools/tma_probe.cu), 128-byte aligned destination, byte counts that match expect_tx, deadlocks.
 // No warp-level primitives: kernels that need lock-step lanes (shuffles, votes, elect) cannot run here.
 #pragma once
 #include <ucontext.h>
@@ -300,7 +300,7 @@ float* emu_smem_ptr(uint32_t addr) {
 }
 static void emu_reduce_complete(const emu::PendingReduce& r) {
   const auto& m = r.map;
-  if (r.c[0] < 0 || r.c[1] < 0 || r.c[2] < 0) emu::fail("TMA reduce with a negative coordinate (traps on B200: tools/tma_reduce_probe.cu)");
+  if (r.c[0] < 0 || r.c[1] < 0 || r.c[2] < 0) emu::fail("TMA reduce with a negative coordinate (traps: tools/tma_reduce_probe.cu)");
   if (((long long)r.c[0] * 4) % 16 != 0) emu::fail("TMA reduce: innermost coordinate not 16-byte aligned");
   const float* src = emu_smem_ptr(r.src);
   if (((size_t)src & 127) != 0) emu::fail("TMA reduce: shared-memory source not 128-byte aligned");
@@ -324,7 +324,7 @@ void emu_bulk_wait(bool) {
   emu::cur->reduces.clear();
 }
 void emu_tma_issue(void* dst, const EmuMap* map, uint64_t* bar, int c0, int c1, int c2) {
-  if (((long long)c0 * 4) % 16 != 0) emu::fail("TMA: innermost coordinate not 16-byte aligned (traps on B200)");
+  if (((long long)c0 * 4) % 16 != 0) emu::fail("TMA: innermost coordinate not 16-byte aligned (traps)");
   if (((size_t)dst & 127) != 0) emu::fail("TMA: shared-memory destination not 128-byte aligned");
   emu::PendingTma t{dst, *map, bar, {c0, c1, c2}};
   if (emu::lazy_tma) emu::pending.push_back(t);

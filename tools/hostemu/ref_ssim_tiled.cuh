@@ -1,5 +1,5 @@
 // tools/hostemu reference (NOT product code): round 1's gather-per-tile SSIM kernel, verified on hardware then, kept as the
-// bit-exact reference the emulator runs ssim_vwalk_kernel (the shipped kernel, 2.4-2.9x faster on B200) against.
+// bit-exact reference the emulator runs ssim_vwalk_kernel (the shipped kernel) against.
 //
 // kornia_b200 -- SSIM index map in one pass (fp32, odd Gaussian window K <= 11, 'reflect' border).
 //
@@ -12,8 +12,8 @@
 //   2. row pass: a thread owns 4 neighbouring outputs of a row, streams the 4+K-1 window positions once,
 //      forms x, y, x*x, y*y, x*y (products rounded on their own, like the reference's img**2 / img1*img2
 //      kernels) and accumulates the five row sums (5*K FMAs per output) into five shared planes;
-//   3. column pass: a thread owns 2 columns x 4 rows and accumulates the five column sums with packed
-//      fma.rn.f32x2 (FFMA2), then evaluates the index with one IEEE rounding per reference op and
+//   3. column pass: a thread owns 2 columns x 4 rows and accumulates the five column sums with
+//      two FMAs per column pair, then evaluates the index with one IEEE rounding per reference op and
 //      stores it.
 // HBM traffic: 8 B read + 4 B written per element.  The kernel is FMA bound (about 5*K*(1+(32+K-1)/32)
 // FMAs per element: 127 for K = 11), not HBM bound.  Tap order (ascending, FMA) is that of the

@@ -1,13 +1,13 @@
 // Executes the kernel templates of kornia_b200/csrc on the CPU (hostemu.h) and compares them BIT FOR BIT with scalar
-// restatements of the same arithmetic.  Covers the kernels written after the round-1 GPU budget was spent (DESIGN.md
-// section 9) and, as a check of the emulator itself, the hardware-verified kernels they derive from.
+// restatements of the same arithmetic.  Covers the pipelined kernels and, as a check of the emulator itself, the
+// kernels they derive from.
 //
 //   make -C tools/hostemu && tools/hostemu/run_emu          (or: python tools/hostemu/run.py)
 //
 // x86 fmaf() is correctly rounded and the build uses -ffp-contract=off, so fp32 results are those of the device
 // intrinsics (__fmaf_rn, __fmul_rn, ...).  What this does NOT cover: timing, occupancy, bank conflicts, the real TMA
 // unit and the memory model of the async proxy -- a pass here means "the index arithmetic, the pipeline bookkeeping and
-// the barriers are consistent", not "runs on a B200".
+// the barriers are consistent", not "runs on the GPU".
 #include "hostemu.h"
 
 #include "../../kornia_b200/csrc/filter2d_tiled.cuh"

@@ -1,8 +1,8 @@
-// Probe (B200): does cudaMemsetAsync on a second stream make progress while a kernel owns every thread slot of every SM, and
+// Probe: does cudaMemsetAsync on a second stream make progress while a kernel owns every thread slot of every SM, and
 // can that kernel see a cuStreamWriteValue32 that follows the memset?  Decides whether the zero-fill of d/dsrc (0.19 ms of the
 // 2.33 ms cfg4 step) can be taken off the critical path with chunked memsets + flags polled by the backward kernel.
 // Every wait in the kernels is bounded by %globaltimer: nothing here can hang the device.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/memset_overlap_probe tools/memset_overlap_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/memset_overlap_probe tools/memset_overlap_probe.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 
