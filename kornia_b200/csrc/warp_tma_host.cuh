@@ -7,10 +7,12 @@ namespace kb200 {
 
 constexpr int TMA_L2_PROMO = 256;  // 256-B L2 promotion on the tensor map (not compared with 128 B on the H100)
 
-// 64 x 32 output tiles, 72 x 40 source box, 2 stages, 2 CTAs per SM: not compared with 3 stages, 96-wide boxes
-// or other tiles on the H100.  On an H100 SXM (700 W) the headline launch runs at 0.73 of the 3.35 TB/s roofline.
+// 64 x 32 output tiles, 72-wide source boxes of 33 to 40 rows, 2 stages, 2 CTAs per SM: not compared with 3 stages, 96-wide
+// boxes or other tiles on the H100.  On an H100 SXM (700 W) the headline launch runs at 0.77 of the 3.35 TB/s roofline
+// (4.95 ms; 5.36 ms with the 40-row box for every tile).  Column-wise walks of bands of strips were measured and lost
+// (DESIGN.md 4.1).
 template <int NC, int INTERP, int PAD, bool PROJ, bool ALIGN, int TW = 64, int TH = 32, int BW = 72, int BH = 40, int NSTAGE = 2, bool DYN = false>
-static int launch_warp_tma(const CUtensorMap& map, const TmaWarpParams& p, cudaStream_t st, int ctas_per_sm = 2) {
+static int launch_warp_tma(const TmaBoxMaps& maps, const TmaWarpParams& p, cudaStream_t st, int ctas_per_sm = 2) {
   auto kern = warp_fwd_tma<NC, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, NSTAGE, DYN>;
   constexpr size_t smem = NSTAGE * (size_t)NC * BW * BH * 4 + 2 * NSTAGE * sizeof(uint64_t) + NSTAGE * sizeof(StageInfo) + NSTAGE * 12 * sizeof(float);
   static unsigned long long configured = 0;  // per instantiation, one bit per device
@@ -24,7 +26,7 @@ static int launch_warp_tma(const CUtensorMap& map, const TmaWarpParams& p, cudaS
     if (!q.counter) return KB200_EUNSUPPORTED;
     q.chunk_tiles = option(OPT_DYN_CHUNK) > 0 ? option(OPT_DYN_CHUNK) : 10;
     q.static_pct = option(OPT_DYN_STATIC);
-    kern<<<grid, TMA_THREADS, smem, st>>>(map, q);
+    kern<<<grid, TMA_THREADS, smem, st>>>(maps, q);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
       set_error("warp_fwd_tma<DYN> launch failed: %s", cudaGetErrorString(e));
@@ -32,7 +34,7 @@ static int launch_warp_tma(const CUtensorMap& map, const TmaWarpParams& p, cudaS
     }
     return KB200_OK;
   }
-  kern<<<grid, TMA_THREADS, smem, st>>>(map, p);
+  kern<<<grid, TMA_THREADS, smem, st>>>(maps, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error("warp_fwd_tma launch failed: %s", cudaGetErrorString(e));
@@ -51,20 +53,27 @@ struct TmaFwdArgs {
   int only_class;  // 0: all samples; CLASS_WIDE / CLASS_SQUARE: only the samples of that footprint class
 };
 
-template <int INTERP>
-static int warp_tma_forward_impl(const TmaFwdArgs& a, cudaStream_t st) {
+// The source as (W, H, B * C) planes, one map per box height of warp_fwd_tma (tma_box_rows); false when the driver refuses.
+template <int BW, int BH>
+static bool encode_box_maps(TmaBoxMaps& maps, const TmaFwdArgs& a) {
   EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
-  CUtensorMap map;
+  if (!encode) return false;
   const cuuint64_t dims[3] = {(cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B * a.C};
   const cuuint64_t strides[2] = {(cuuint64_t)a.W * 4, (cuuint64_t)a.H * a.W * 4};
-  const cuuint32_t box[3] = {72, 40, (cuuint32_t)a.C};
   const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult cr = encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(a.src), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return KB200_EUNSUPPORTED;
+  for (int i = 0; i < TMA_BOX_HEIGHTS; ++i) {
+    const cuuint32_t box[3] = {(cuuint32_t)BW, (cuuint32_t)tma_box_rows(BH, i), 1};
+    if (encode(&maps.map[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(a.src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return false;
+  }
+  return true;
+}
+
+template <int INTERP>
+static int warp_tma_forward_impl(const TmaFwdArgs& a, cudaStream_t st) {
+  TmaBoxMaps map;
+  if (!encode_box_maps<72, 40>(map, a)) return KB200_EUNSUPPORTED;
   TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr, 0, 0};
   const int C = a.C, pad = a.pad;
   const bool projective = a.projective != 0, align = a.align != 0;

@@ -11,7 +11,7 @@ namespace kb200 {
 constexpr int SQ_TW = 32, SQ_TH = 32, SQ_BW = 56, SQ_BH = 56, SQ_STAGES = 2, SQ_CTAS = 2;
 
 template <int NC, int PAD>
-static int launch_square(const CUtensorMap& map, const TmaWarpParams& p, bool projective, bool align, cudaStream_t st) {
+static int launch_square(const TmaBoxMaps& map, const TmaWarpParams& p, bool projective, bool align, cudaStream_t st) {
   if (projective)
     return align ? launch_warp_tma<NC, KB200_BILINEAR, PAD, true, true, SQ_TW, SQ_TH, SQ_BW, SQ_BH, SQ_STAGES>(map, p, st, SQ_CTAS)
                  : launch_warp_tma<NC, KB200_BILINEAR, PAD, true, false, SQ_TW, SQ_TH, SQ_BW, SQ_BH, SQ_STAGES>(map, p, st, SQ_CTAS);
@@ -21,17 +21,8 @@ static int launch_square(const CUtensorMap& map, const TmaWarpParams& p, bool pr
 
 int warp_tma_forward_square(const TmaFwdArgs& a, cudaStream_t st) {
   if (a.C != 1 && a.C != 3) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
-  CUtensorMap map;
-  const cuuint64_t dims[3] = {(cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B * a.C};
-  const cuuint64_t strides[2] = {(cuuint64_t)a.W * 4, (cuuint64_t)a.H * a.W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)SQ_BW, (cuuint32_t)SQ_BH, (cuuint32_t)a.C};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult cr = encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(a.src), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return KB200_EUNSUPPORTED;
+  TmaBoxMaps map;
+  if (!encode_box_maps<SQ_BW, SQ_BH>(map, a)) return KB200_EUNSUPPORTED;
   const TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr, 0, 0};
   const bool projective = a.projective != 0, align = a.align != 0;
 #define KB_SQ_CASE(NC_, PAD_) \

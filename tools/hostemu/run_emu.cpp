@@ -392,6 +392,14 @@ static void test_remap_piped(int B, int H, int W, int h, int w, unsigned grid, b
 }
 
 // ------------------------------------------------------------------------------------------ tiled warp forward (the headline kernel)
+// the source as (W, H, planes), one map per box height of warp_fwd_tma (boxes of one plane, BW wide)
+template <int BW, int BH>
+static TmaBoxMaps box_maps(const float* src, int W, int H, int planes) {
+  TmaBoxMaps maps;
+  for (int i = 0; i < TMA_BOX_HEIGHTS; ++i) maps.map[i] = emu::make_map(src, W, H, planes, BW, tma_box_rows(BH, i), 1);
+  return maps;
+}
+
 template <bool PROJ, int PAD, int TW, int TH, int BW, int BH, int INTERP = KB200_BILINEAR, bool ALIGN = true>
 static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool lazy, bool tame) {
   emu::lazy_tma = lazy;
@@ -426,7 +434,7 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
                                                           PROJ ? mm[7] * by[y] : 0.f, mm[2], mm[5], mm[8]);
       }
   p.out = o1;
-  const CUtensorMap map = emu::make_map(src, W, H, B * C, BW, BH, C);
+  const TmaBoxMaps map = box_maps<BW, BH>(src, W, H, B * C);
   emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2>(map, p); });
   if (INTERP == KB200_BILINEAR && TW == 64) {  // the run-time work distribution: same tiles, same results
     std::vector<float> o3s;
@@ -798,7 +806,7 @@ static void probe_forward() {
   const float fillc[3] = {0.25f, 0.5f, 0.75f};
   p.src = src; p.m = M; p.bx = bx.data(); p.by = by.data(); p.fill = fillc; p.out = o1;
   p.B = 1; p.H = H; p.W = W; p.h = H; p.w = W; p.Bm = 1; p.align = 1; p.only_class = 0;
-  const CUtensorMap map = emu::make_map(src, W, H, C, 72, 40, C);
+  const TmaBoxMaps map = box_maps<72, 40>(src, W, H, C);
   emu_careful_pixels = emu_inner_tiles = emu_other_tiles = 0;
   emu::launch(4, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, true, true, 64, 32, 72, 40, 2>(map, p); });
   printf("interp=%d pad=%d: tiles INNER %lld other %lld (each counted once per CTA), pixels on the exact path %lld of %d\n", INTERP, PAD, emu_inner_tiles, emu_other_tiles,
