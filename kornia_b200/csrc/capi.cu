@@ -28,26 +28,39 @@ void set_error(const char* fmt, ...) {
 }
 
 // ---------------------------------------------------------------- kernel-selection switches (common.cuh: enum Option)
-static const char* const OPTION_NAMES[OPT_COUNT] = {"tma", "tiled_filter", "square_tiles", "sep_vwalk", "tiled_gradient", "u8_tiled", "bwd_stride1", "remap_piped", "dyn_sched", "dyn_chunk", "dyn_static"};
-// sep_vwalk 0 and remap_piped 0: on an H100 SXM (700 W) the band walk lost to the tiled blur at 5-13 taps and tied at 17
-// (tools/ab_blur.py, B=256), and the pipelined remap lost 6-14 % with per-sample maps and tied with a shared map (tools/ab_remap.py, B=64)
-static const int OPTION_DEFAULTS[OPT_COUNT] = {1, 1, 1, 0, 1, 1, 1, 0, 1, 10, 85};
+// One row per switch, keyed by its enum value: the loader and the name lookup never depend on the order of the rows.
+static const struct {
+  Option opt;
+  const char* name;
+  int value;  // default, unless KB200_<NAME> is set
+} OPTIONS[] = {
+    {OPT_TMA, "tma", 1},
+    {OPT_TILED_FILTER, "tiled_filter", 1},
+    {OPT_SQUARE_TILES, "square_tiles", 1},
+    {OPT_TILED_GRADIENT, "tiled_gradient", 1},
+    {OPT_U8_TILED, "u8_tiled", 1},
+    {OPT_BWD_STRIDE1, "bwd_stride1", 1},
+    {OPT_DYN_SCHED, "dyn_sched", 1},
+    {OPT_DYN_CHUNK, "dyn_chunk", 10},
+    {OPT_DYN_STATIC, "dyn_static", 85},
+};
+static_assert(sizeof(OPTIONS) / sizeof(OPTIONS[0]) == OPT_COUNT, "one OPTIONS row per Option");
 static int g_options[OPT_COUNT];
 static const bool g_options_ready = [] {  // once, when the library is loaded: KB200_<NAME>=<int> overrides the default
-  for (int i = 0; i < OPT_COUNT; ++i) {
+  for (const auto& row : OPTIONS) {
     char env[64] = "KB200_";
     size_t n = strlen(env);
-    for (const char* c = OPTION_NAMES[i]; *c && n + 1 < sizeof(env); ++c) env[n++] = (char)((*c >= 'a' && *c <= 'z') ? *c - 32 : *c);
+    for (const char* c = row.name; *c && n + 1 < sizeof(env); ++c) env[n++] = (char)((*c >= 'a' && *c <= 'z') ? *c - 32 : *c);
     env[n] = 0;
     const char* v = getenv(env);
-    g_options[i] = (v && v[0]) ? atoi(v) : OPTION_DEFAULTS[i];
+    g_options[row.opt] = (v && v[0]) ? atoi(v) : row.value;
   }
   return true;
 }();
 int option(Option o) { return __atomic_load_n(&g_options[o], __ATOMIC_RELAXED); }
 static int option_index(const char* name) {
-  for (int i = 0; name && i < OPT_COUNT; ++i)
-    if (strcmp(name, OPTION_NAMES[i]) == 0) return i;
+  for (const auto& row : OPTIONS)
+    if (name && strcmp(name, row.name) == 0) return row.opt;
   return -1;
 }
 
@@ -499,9 +512,6 @@ int kb200_sepfilter_forward(const void* x, const void* kernel_x, const void* ker
   KB_CHECK_ARG((long long)B * C <= MAX_Z, "B*C = %lld planes exceed the %d-plane launch limit", (long long)B * C, MAX_Z);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == KB200_F32) {
-    rc = sepfilter_vwalk_forward((const float*)x, (const float*)kernel_x, (const float*)kernel_y, (float*)out, B, C, H, W, Bkx,
-                                 kw, Bky, kh, border, same, st);  // opt-in (KB200_SEP_VWALK=1), declines otherwise
-    if (rc != KB200_EUNSUPPORTED) return rc;
     rc = sepfilter_tiled_forward((const float*)x, (const float*)kernel_x, (const float*)kernel_y, (float*)out, B, C, H, W, Bkx,
                                  kw, Bky, kh, border, same, st);
     if (rc != KB200_EUNSUPPORTED) return rc;
@@ -582,9 +592,6 @@ int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void
     return KB200_EUNSUPPORTED;
   }
   const float w = (float)weight;
-  rc = sepfilter_vwalk_forward((const float*)x, (const float*)kernel_x, (const float*)kernel_y, (float*)out, B, C, H, W, Bkx, kw, Bky, kh,
-                               border, same, (cudaStream_t)stream, &w);  // opt-in (KB200_SEP_VWALK=1), declines otherwise
-  if (rc != KB200_EUNSUPPORTED) return rc;
   rc = sepfilter_tiled_forward((const float*)x, (const float*)kernel_x, (const float*)kernel_y, (float*)out, B, C, H, W, Bkx, kw, Bky,
                                kh, border, same, (cudaStream_t)stream, &w);
   if (rc == KB200_EUNSUPPORTED) set_error("the fused filter + lerp kernel covers square odd kernels up to 11 taps, 'same', non-circular borders");

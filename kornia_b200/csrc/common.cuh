@@ -81,16 +81,16 @@ __device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
 // ---------------------------------------------------------------- kernel-selection switches (capi.cu)
 // Which of the library's own kernels serves a request.  Every switch is read from the environment ONCE, when the library is
 // loaded (KB200_<NAME>=0|1), and can be changed afterwards through kb200_set_option (tests compare a tiled kernel with the
-// kernel it stands in for): no getenv on the call path.  -1 = automatic (the dispatcher's own rule).
+// kernel it stands in for): no getenv on the call path.
 enum Option {
   OPT_TMA,             // TMA-tiled warp / remap / backward kernels (off: the generic per-pixel kernels)
   OPT_TILED_FILTER,    // shared-memory filter kernels (off: filter_generic.cuh)
   OPT_SQUARE_TILES,    // second tile shape of the forward warp for rotated samples
-  OPT_SEP_VWALK,       // band-walking separable filter: -1 auto (11 taps and more), 0 never, 1 whenever it applies
   OPT_TILED_GRADIENT,  // shared-memory derivative stencils (off: gradient.cuh)
   OPT_U8_TILED,        // staged-window uint8 ingest warp (off: per-tap kernel)
-  OPT_BWD_STRIDE1,     // tiled backward on stride-1 lanes (default; 0: the column-pair lanes, 5 % slower at cfg4)
-  OPT_REMAP_PIPED,     // remap on the pipelined persistent kernel (off: one CTA per tile)
+  OPT_BWD_STRIDE1,     // tiled backward on stride-1 lanes (default; 0: the column-pair lanes, dealt out in advance).  At cfg4
+                       // the column pairs were 5 % slower on a B200; on an H100 SXM at 400 W, one alternated A/B had them
+                       // 2.6 % faster (4.69 vs 4.81 ms per launch).  The default has not been chosen again.
   OPT_DYN_SCHED,       // headline warp: strips handed out at run time in chunks (off: dealt out in advance)
   OPT_DYN_CHUNK,       // tiles per chunk of the run-time work distribution (forward kernel)
   OPT_DYN_STATIC,      // percent of the full rounds of strips still dealt out in advance by the DYN forward kernel

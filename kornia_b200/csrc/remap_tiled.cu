@@ -1,5 +1,5 @@
 // kornia_b200 -- host dispatch of the tiled remap forward kernel.
-#include "remap_piped.cuh"
+#include "remap_tiled.cuh"
 
 namespace kb200 {
 
@@ -19,78 +19,12 @@ static int launch_remap_tiled(const CUtensorMap& map, const RemapTiledParams& p,
   return KB200_OK;
 }
 
-template <int NC, int PAD, bool ALIGN>
-static int launch_remap_piped(const CUtensorMap& msrc, const CUtensorMap& mmx, const CUtensorMap& mmy, const RemapTiledParams& p, cudaStream_t st) {
-  auto kern = remap_piped_kernel<NC, PAD, ALIGN>;
-  constexpr size_t smem = (size_t)REMAP_PIPED_STAGES * ((size_t)NC * 72 * 40 * 4 + 2 * 64 * 32 * 4 + TMA_CONSUMER_WARPS * 16) +
-                          5 * REMAP_PIPED_STAGES * sizeof(uint64_t) +
-                          REMAP_PIPED_STAGES * sizeof(StageInfo) + 64;
-  static unsigned long long configured = 0;  // per instantiation, one bit per device
-  KB_SET_SMEM_ONCE(configured, kern, smem);
-  const long long nstrips = (long long)p.B * ceil_div(p.h, 32), cap = 2ll * sm_count();
-  kern<<<(int)(nstrips < cap ? nstrips : cap), TMA_THREADS, smem, st>>>(msrc, mmx, mmy, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("remap_piped launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
-}
-
-// The pipelined kernel (remap_piped.cuh): maps must be TMA-addressable (w % 4 == 0, 16-byte aligned); switch remap_piped.
-int remap_piped_forward(const float* src, const float* map_x, const float* map_y, float* out, int B, int C, int H, int W, int h, int w,
-                        int Bmap, int normalized, int pad, int align, cudaStream_t st) {
-  if (!option(OPT_REMAP_PIPED)) return KB200_EUNSUPPORTED;
-  // under 'reflection' this kernel is not reliably faster than the one-CTA-per-tile kernel, which therefore keeps that mode
-  if (pad == KB200_REFLECTION && option(OPT_REMAP_PIPED) < 2) return KB200_EUNSUPPORTED;  // remap_piped = 2: measure it anyway
-  if ((w % 4) != 0 || ((reinterpret_cast<uintptr_t>(map_x) | reinterpret_cast<uintptr_t>(map_y)) & 15) != 0) return KB200_EUNSUPPORTED;
-  if ((long long)B * ceil_div(h, 32) > 0x7fffffffll || (long long)B * C > 0x7fffffffll) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMap msrc, mmx, mmy;
-  {
-    const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * C};
-    const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-    const cuuint32_t box[3] = {72, 40, (cuuint32_t)C};
-    if (encode(&msrc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
-  {
-    const cuuint64_t dims[3] = {(cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)Bmap};
-    const cuuint64_t strides[2] = {(cuuint64_t)w * 4, (cuuint64_t)h * w * 4};
-    const cuuint32_t box[3] = {64, 32, 1};
-    if (encode(&mmx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(map_x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS ||
-        encode(&mmy, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(map_y), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
-  RemapTiledParams p{src, map_x, map_y, out, B, H, W, h, w, Bmap, normalized, nullptr};
-#define KB_REMAP_CASE(NC_, PAD_)                                                                                   \
-  if (C == NC_ && pad == PAD_)                                                                                     \
-    return align ? launch_remap_piped<NC_, PAD_, true>(msrc, mmx, mmy, p, st) : launch_remap_piped<NC_, PAD_, false>(msrc, mmx, mmy, p, st);
-  KB_REMAP_CASE(3, KB200_ZEROS)
-  KB_REMAP_CASE(3, KB200_BORDER)
-  KB_REMAP_CASE(3, KB200_REFLECTION)
-  KB_REMAP_CASE(1, KB200_ZEROS)
-  KB_REMAP_CASE(1, KB200_BORDER)
-  KB_REMAP_CASE(1, KB200_REFLECTION)
-#undef KB_REMAP_CASE
-  return KB200_EUNSUPPORTED;
-}
-
 // KB200_EUNSUPPORTED -> the caller runs the generic kernel.
 int remap_tiled_forward(const float* src, const float* map_x, const float* map_y, float* out, int B, int C, int H, int W, int h, int w,
                         int Bmap, int normalized, int interp, int pad, int align, cudaStream_t st) {
   if (!option(OPT_TMA)) return KB200_EUNSUPPORTED;
   if (interp != KB200_BILINEAR || (C != 1 && C != 3) || pad == KB200_FILL) return KB200_EUNSUPPORTED;
   if ((W % 4) != 0 || (reinterpret_cast<uintptr_t>(src) & 15) != 0) return KB200_EUNSUPPORTED;
-  {
-    const int rc = remap_piped_forward(src, map_x, map_y, out, B, C, H, W, h, w, Bmap, normalized, pad, align, st);
-    if (rc != KB200_EUNSUPPORTED) return rc;
-  }
   if (B > 65535 || ceil_div(h, 32) > 65535) return KB200_EUNSUPPORTED;
   EncodeTiledFn encode = encode_tiled_fn();
   if (!encode) return KB200_EUNSUPPORTED;

@@ -231,8 +231,4 @@ __global__ void __launch_bounds__(256, 3) sepfilter_tiled_kernel(const __grid_co
 int sepfilter_tiled_forward(const float* x, const float* kx, const float* ky, float* out, int B, int C, int H, int W, int Bkx, int kw,
                             int Bky, int kh, int border, int same, cudaStream_t st, const float* lerp_w = nullptr);
 
-// Band-walking variant (sepfilter_vwalk.cuh), opt-in with KB200_SEP_VWALK=1; KB200_EUNSUPPORTED -> sepfilter_tiled_forward.
-int sepfilter_vwalk_forward(const float* x, const float* kx, const float* ky, float* out, int B, int C, int H, int W, int Bkx, int kw,
-                            int Bky, int kh, int border, int same, cudaStream_t st, const float* lerp_w = nullptr);
-
 }  // namespace kb200

@@ -2,7 +2,7 @@
 //
 // Same arithmetic as ssim_tiled_kernel (ssim_tiled.cuh: products rounded on their own, five row sums with ascending
 // FMA taps, five column sums on column pairs (two FFMAs per pair), the index with one rounding per reference op of
-// kornia/metrics/ssim.py:92-139 -- bit-identical results), on the walk of sepfilter_vwalk_kernel.  The first version
+// kornia/metrics/ssim.py:92-139 -- bit-identical results), with persistent CTAs walking column bands.  The first version
 // gathers both boxes with scalar loads, synchronises, row-filters 32 + K - 1 rows, synchronises, column-filters: one
 // tile per CTA, nothing overlaps, measured 6.6 ms at B=64x3x1080x1920 (11 % of the HBM roofline, ~20 % of its FMA
 // bound; DESIGN.md 4.5).  Here persistent CTAs walk 64-column bands top to bottom:

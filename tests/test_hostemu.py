@@ -19,7 +19,7 @@ def test_kernels_on_the_host_emulator():
     run = subprocess.run([os.path.join(EMU, "run_emu")], capture_output=True, text=True, timeout=600)
     tail = run.stdout[-3000:] + run.stderr[-2000:]
     assert run.returncode == 0 and "PASSED: 0 failing comparisons" in run.stdout, tail
-    for kernel in ("sepfilter_tiled_kernel", "sepfilter_vwalk_kernel", "filter2d_tiled_kernel<5, DOWN2>", "grad_tiled_kernel", "ssim_vwalk_kernel",
+    for kernel in ("sepfilter_tiled_kernel", "sepfilter_tiled_kernel<LERP>", "filter2d_tiled_kernel<5, DOWN2>", "grad_tiled_kernel", "ssim_vwalk_kernel",
                    "remap_tiled_kernel<LENS>", "warp_bwd_tma2 (per-warp pipelines", "warp_fwd_tma (headline",
                    "warp_fwd_u8hwc", "warp_u8_tiled_kernel vs warp_fwd_u8hwc", "unit_from_byte == float(u) / 255.0f for all 256 bytes"):
         assert kernel in run.stdout, kernel

@@ -386,10 +386,13 @@ def test_prelude_keeps_autograd_path():
 @pytest.mark.parametrize("border", ["constant", "reflect", "replicate"])
 @pytest.mark.parametrize("k", [3, 5, 7, 9, 11, 13, 15, 17])
 def test_tiled_sepfilter_bit_identical_to_generic(k, border):
-    import os
-
+    """Per-sample taps exercise the b % Bk indexing; 37 x 3 x 200 x 520 has more strips than the persistent grid has CTAs."""
     g = torch.Generator().manual_seed(k)
-    for (B, C, H, W) in ((2, 3, 70, 200), (1, 1, 32, 128), (3, 2, 45, 132), (1, 3, 9 + k, 12 + 4 * (k // 4))):
+    shapes = ((2, 3, 70, 200), (1, 1, 32, 128), (3, 2, 45, 132), (1, 3, 9 + k, 12 + 4 * (k // 4)), (3, 2, 33, 4), (1, 1, 6, 8),
+              (2, 3, 1080, 1920), (37, 3, 200, 520))
+    for (B, C, H, W) in shapes:
+        if border != "constant" and min(H, W) <= k // 2:  # a fold needs an image larger than the half-width
+            continue
         x = torch.rand(B, C, H, W, generator=g).to(DEV)
         kx = torch.randn(B, k, generator=g).to(DEV)
         ky = torch.randn(1, k, generator=g).to(DEV)
@@ -535,14 +538,11 @@ def test_tiled_filter2d_bit_identical_to_generic(k, border):
                 torch.testing.assert_close(a.cpu(), want, rtol=1e-4, atol=1e-5)
 
 
-@pytest.mark.parametrize("piped", [0, 1])
 @pytest.mark.parametrize("pad", ["zeros", "border", "reflection"])
 @pytest.mark.parametrize("ac", [None, True])
 @pytest.mark.parametrize("C", [3, 1])
-def test_tiled_remap_bit_identical_to_generic(piped, pad, ac, C):
-    """Smooth maps (served from the staged box), a noisy map (mostly exact path), out-of-view and NaN entries; both tiled kernels
-    (one CTA per tile / the pipelined persistent kernel, switch remap_piped)."""
-    K.config.set("remap_piped", piped)
+def test_tiled_remap_bit_identical_to_generic(pad, ac, C):
+    """Smooth maps (served from the staged box), a noisy map (mostly exact path), out-of-view and NaN entries."""
     H, W, h, w = 96, 160, 80, 136
     g = torch.Generator().manual_seed(4)
     img = torch.rand(3, C, H, W, generator=g).to(DEV)
@@ -566,9 +566,9 @@ def test_tiled_remap_bit_identical_to_generic(piped, pad, ac, C):
 
 
 @pytest.mark.parametrize("pad", ["zeros", "reflection"])
-def test_piped_remap_many_strips(pad):
-    """More strips than persistent CTAs (segments start inside strips, every buffer is reused many times), per-sample and shared
-    maps, normalised coordinates: the pipelined kernel against the one-CTA-per-tile kernel, bit for bit."""
+def test_tiled_remap_many_strips(pad):
+    """A batch of many tiles with per-sample and shared maps and normalised coordinates: the tiled kernel against the generic
+    kernel, bit for bit, in one launch."""
     B, H, W = 40, 200, 264   # 40 x 7 = 280 strips of 5 tiles
     g = torch.Generator().manual_seed(11)
     img = torch.rand(B, 3, H, W, generator=g).to(DEV)
@@ -577,12 +577,10 @@ def test_piped_remap_many_strips(pad):
     mx = (xs[None] + amp * torch.sin(ys / 17.0)[None] - 2.0).contiguous().to(DEV)
     my = (ys[None] + amp * torch.cos(xs / 23.0)[None] + 1.5).contiguous().to(DEV)
     for (ax, ay, norm) in ((mx, my, False), (mx[:1], my[:1], False), (2 * mx / (W - 1) - 1, 2 * my / (H - 1) - 1, True)):
-        with K.config.override(remap_piped=0):
-            want = K.remap(img, ax, ay, padding_mode=pad, align_corners=True, normalized_coordinates=norm)
-        with K.config.override(remap_piped=1):
-            n0 = K._ops.launch_count
-            got = K.remap(img, ax, ay, padding_mode=pad, align_corners=True, normalized_coordinates=norm)
-            assert K._ops.launch_count - n0 == 1
+        want = _generic(lambda: K.remap(img, ax, ay, padding_mode=pad, align_corners=True, normalized_coordinates=norm), check_variant=False)
+        n0 = K._ops.launch_count
+        got = K.remap(img, ax, ay, padding_mode=pad, align_corners=True, normalized_coordinates=norm)
+        assert K._ops.launch_count - n0 == 1
         assert torch.equal(got, want), float((got - want).abs().max())
 
 

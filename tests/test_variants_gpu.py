@@ -79,56 +79,6 @@ def test_tiled_sobel_bit_identical_and_golden(shape):
         torch.testing.assert_close(res.cpu(), outs["out"], rtol=1e-4, atol=1e-5)
 
 
-# ------------------------------------------------------------------------------------------ band-walking separable filter
-_VWALK_SHAPES = [(2, 3, 70, 132), (1, 1, 32, 128), (3, 2, 33, 4), (1, 2, 97, 260), (1, 1, 6, 8), (2, 3, 1080, 1920)]
-
-
-@pytest.mark.parametrize("border,ksize,shape", [(b, k, s) for b in ("reflect", "replicate", "constant") for k in (3, 5, 11, 17) for s in _VWALK_SHAPES
-                                                if b == "constant" or min(s[-2:]) > k // 2])  # a fold needs an image larger than the half-width
-def test_band_walk_separable_filter_bit_identical(border, ksize, shape):
-    """sepfilter_vwalk_kernel (KB200_SEP_VWALK=1) == sepfilter_tiled_kernel, bit for bit: same taps, same FMA order, the
-    vertical fold applied to row-filtered rows instead of input rows.  Per-sample taps exercise the b % Bk indexing."""
-    g = torch.Generator().manual_seed(ksize)
-    x = torch.rand(*shape, device=DEV)
-    kx = torch.rand(shape[0], ksize, generator=g).to(DEV)
-    ky = torch.rand(1, ksize, generator=g).to(DEV)
-    K.config.set("sep_vwalk", 0)
-    want = K.filter2d_separable(x, kx, ky, border)
-    K.config.set("sep_vwalk", 1)
-    got = K.filter2d_separable(x, kx, ky, border)
-    assert torch.equal(got, want), float((got - want).abs().max())
-
-
-@pytest.mark.parametrize("border", ["reflect", "replicate", "constant"])
-@pytest.mark.parametrize("ksize,shape", [(3, (2, 3, 70, 132)), (5, (1, 1, 32, 128)), (11, (1, 2, 97, 260)), (7, (2, 3, 1080, 1920))])
-def test_band_walk_unsharp_mask_bit_identical(border, ksize, shape):
-    """unsharp_mask through the lerp epilogue of the band-walking kernel == through the strip-walking one."""
-    x = torch.rand(*shape, device=DEV)
-    K.config.set("sep_vwalk", 0)
-    want = K.filters.unsharp_mask(x, (ksize, ksize), (1.5, 1.5), border)
-    K.config.set("sep_vwalk", 1)
-    got = K.filters.unsharp_mask(x, (ksize, ksize), (1.5, 1.5), border)
-    assert torch.equal(got, want), float((got - want).abs().max())
-
-
-def test_band_walk_many_segments_and_blur_golden():
-    """More bands than CTAs (leftover bands are cut into runs: segments that start in the middle of a band), and the
-    gaussian_blur2d goldens of the reference through the new kernel."""
-    K.config.set("sep_vwalk", 1)
-    x = torch.rand(37, 3, 200, 520, device=DEV)   # 111 planes x 5 bands = 555 bands > 444 CTAs
-    got = K.gaussian_blur2d(x, (11, 11), (2.0, 2.0))
-    K.config.set("sep_vwalk", 0)
-    assert torch.equal(got, K.gaussian_blur2d(x, (11, 11), (2.0, 2.0)))
-    K.config.set("sep_vwalk", 1)
-    FIL = golden("filter")
-    for name in FIL.names("gaussian_blur2d"):
-        op, kw, ins, outs = FIL.case(name)
-        sigma = ins["sigma"].to(DEV) if "sigma" in ins else tuple(kw["sigma"])
-        res = K.gaussian_blur2d(ins["input"].to(DEV), tuple(kw["kernel_size"]) if isinstance(kw["kernel_size"], list) else kw["kernel_size"],
-                                sigma, kw["border_type"], kw["separable"])
-        torch.testing.assert_close(res.cpu(), outs["out"], rtol=1e-4, atol=1e-5)
-
-
 # ------------------------------------------------------------------------------------------ band-walking SSIM
 @pytest.mark.parametrize("window,shape", [(w, s) for w in (3, 5, 7, 9, 11)
                                           for s in ((2, 3, 70, 132), (1, 1, 32, 64), (3, 2, 33, 8), (1, 2, 97, 260), (1, 1, 6, 8), (1, 3, 1080, 1920))

@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(256, 2) ssim_tiled_kernel(const __grid_constan
 
 int ssim_tiled_forward(const float* a, const float* b, const float* taps, float* out, int planes, int H, int W, int K, float C1,
                        float C2, float eps, cudaStream_t st);
-// Band-walking TMA variant (ssim_vwalk.cuh), opt-in with KB200_SSIM_VWALK=1; KB200_EUNSUPPORTED -> ssim_tiled_forward.
+// The library's SSIM kernel (ssim_vwalk.cuh, band-walking with TMA); KB200_EUNSUPPORTED outside its envelope.
 int ssim_vwalk_forward(const float* a, const float* b, const float* taps, float* out, int planes, int H, int W, int K, float C1, float C2,
                        float eps, cudaStream_t st);
 
