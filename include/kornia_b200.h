@@ -55,7 +55,8 @@ const char* kb200_last_warp_variant(void);
  * samples, 32x32 tiles for rotated / sheared ones; each kernel skips the other's samples). */
 int kb200_last_warp_launches(void);
 /* Kernel-selection switches: which of the library's own kernels serves a request.  Names: "tma", "tiled_filter",
- * "square_tiles", "tiled_gradient", "u8_tiled", "bwd_stride1", "dyn_sched", "dyn_chunk" (tiles), "dyn_static" (percent);
+ * "square_tiles", "tiled_gradient", "u8_tiled", "bwd_stride1", "dyn_sched", "dyn_chunk" (tiles), "dyn_static" (percent),
+ * "sweep" (forward under "dyn_sched": tiles drawn in raster order; 0 = the strip deal of "dyn_chunk" / "dyn_static");
  * values 0 = off, 1 = on.
  * Each is initialised ONCE when the library is loaded (environment KB200_<NAME>, else the built-in default); there is no
  * getenv on the call path.  The parity tests use the setter to run a tiled kernel against the kernel it stands in for.

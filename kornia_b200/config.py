@@ -10,8 +10,10 @@ Device-side (forwarded to the C library): ``tma`` (TMA-tiled warp / remap / back
 kernels), ``tiled_filter`` (shared-memory filter kernels; off = generic), ``square_tiles`` (second forward tile shape for
 rotated samples), ``tiled_gradient``, ``u8_tiled`` (staged-window uint8 ingest warp; off = per-tap kernel), ``bwd_stride1``
 (tiled backward on stride-1 lanes; off = column-pair lanes), ``dyn_sched`` (warp forward and backward: the last rounds of strips /
-every warp's work drawn at run time from a per-device ring of counters; off = dealt out in advance), ``dyn_chunk`` (tiles per
-chunk, 10), ``dyn_static`` (percent of the full rounds the forward kernel still deals out in advance, 85).
+every warp's work drawn at run time from a per-device ring of counters; off = dealt out in advance), ``sweep`` (forward kernel
+under ``dyn_sched``: every run of tiles drawn in raster order, so the grid sweeps each image as one band; off = the strip deal
+of the next two switches), ``dyn_chunk`` (tiles per chunk of the strip deal, 10), ``dyn_static`` (percent of the full rounds
+the strip deal hands out in advance, 85).
 Host-side: ``fused_pyrdown`` (5x5 blur + 2x decimation in one kernel), ``fused_undistort`` (lens model evaluated inside
 the sampling kernel), ``fast_filter_bwd`` (input gradient of the separable filter through the one-pass forward kernel),
 ``torch_prelude`` (the (B,3,3) matrix chain as the reference's torch op sequence instead of one launch; needed for double
@@ -24,7 +26,8 @@ import os
 
 from . import _lib
 
-DEVICE_OPTIONS = ("tma", "tiled_filter", "square_tiles", "tiled_gradient", "u8_tiled", "bwd_stride1", "dyn_sched", "dyn_chunk", "dyn_static")
+DEVICE_OPTIONS = ("tma", "tiled_filter", "square_tiles", "tiled_gradient", "u8_tiled", "bwd_stride1", "dyn_sched", "dyn_chunk", "dyn_static",
+                  "sweep")
 _HOST_DEFAULTS = {"fused_pyrdown": 1, "fused_undistort": 1, "fast_filter_bwd": 1, "torch_prelude": 0}
 
 

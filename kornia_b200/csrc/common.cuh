@@ -94,6 +94,7 @@ enum Option {
   OPT_DYN_SCHED,       // headline warp: strips handed out at run time in chunks (off: dealt out in advance)
   OPT_DYN_CHUNK,       // tiles per chunk of the run-time work distribution (forward kernel)
   OPT_DYN_STATIC,      // percent of the full rounds of strips still dealt out in advance by the DYN forward kernel
+  OPT_SWEEP,           // DYN forward kernel: every run of tiles drawn in raster order (off: the strip deal of dyn_chunk / dyn_static)
   OPT_COUNT
 };
 int option(Option o);

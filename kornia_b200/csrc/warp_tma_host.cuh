@@ -8,9 +8,10 @@ namespace kb200 {
 constexpr int TMA_L2_PROMO = 256;  // 256-B L2 promotion on the tensor map (not compared with 128 B on the H100)
 
 // 64 x 32 output tiles, 72-wide source boxes of 33 to 40 rows, 2 stages, 2 CTAs per SM: not compared with 3 stages, 96-wide
-// boxes or other tiles on the H100.  On an H100 SXM (700 W) the headline launch runs at 0.77 of the 3.35 TB/s roofline
-// (4.95 ms; 5.36 ms with the 40-row box for every tile).  Column-wise walks of bands of strips were measured and lost
-// (DESIGN.md 4.1).
+// boxes or other tiles on the H100.  On an H100 SXM (700 W) the headline launch ran at 0.77 of the 3.35 TB/s roofline under
+// the strip deal (4.95 ms; 5.36 ms with the 40-row box for every tile).  DYN launches run the sweep by default (every tile
+// drawn in raster order): on an H100 held to 400 W, 4.47-4.55 ms against 4.95-4.97 ms for the strip deal.  Column-wise walks
+// of bands of strips were measured and lost (DESIGN.md 4.1).
 template <int NC, int INTERP, int PAD, bool PROJ, bool ALIGN, int TW = 64, int TH = 32, int BW = 72, int BH = 40, int NSTAGE = 2, bool DYN = false>
 static int launch_warp_tma(const TmaBoxMaps& maps, const TmaWarpParams& p, cudaStream_t st, int ctas_per_sm = 2) {
   auto kern = warp_fwd_tma<NC, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, NSTAGE, DYN>;
@@ -24,8 +25,13 @@ static int launch_warp_tma(const TmaBoxMaps& maps, const TmaWarpParams& p, cudaS
     TmaWarpParams q = p;
     q.counter = take_work_counter(st);
     if (!q.counter) return KB200_EUNSUPPORTED;
-    q.chunk_tiles = option(OPT_DYN_CHUNK) > 0 ? option(OPT_DYN_CHUNK) : 10;
-    q.static_pct = option(OPT_DYN_STATIC);
+    if (option(OPT_SWEEP)) {  // every run drawn, in raster order (warp_fwd_tma: the producer)
+      q.chunk_tiles = SWEEP_TILES;
+      q.static_pct = 0;
+    } else {
+      q.chunk_tiles = option(OPT_DYN_CHUNK) > 0 ? option(OPT_DYN_CHUNK) : 10;
+      q.static_pct = option(OPT_DYN_STATIC);
+    }
     kern<<<grid, TMA_THREADS, smem, st>>>(maps, q);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

@@ -6,7 +6,8 @@ ceiling, interleaved in one process; bit comparison first.
 An ARM is ``name=value[,name=value...]`` (device switches of kornia_b200.config, applied around the call), ``default`` (the
 switches as loaded) or ``copy`` (``out.copy_(src)`` on tensors of the workload's size: the same 24 B per pixel a warp moves).
 Every warp arm is checked with torch.equal against the first one.  Kernel time comes from CUDA events around each forward
-launch (the same events bench.py's roofline.kernel_ms uses); each repeat of each arm is the mean of --steps launches."""
+launch (the same events bench.py's roofline.kernel_ms uses); each repeat of each arm is the mean of --steps launches, and the
+arms take turns in an order that rotates from repeat to repeat."""
 import argparse
 import os
 import statistics
@@ -23,7 +24,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=256)
 ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--steps", type=int, default=20)
-ap.add_argument("arms", nargs="*", default=["default", "dyn_static=0", "dyn_sched=0", "copy"])
+ap.add_argument("arms", nargs="*", default=["default", "sweep=0", "dyn_sched=0", "copy"])
 args = ap.parse_args()
 
 try:
@@ -90,9 +91,13 @@ def timed(arm):
 
 res = {a: [] for a in args.arms}
 for rep in range(args.reps):
-    for arm in args.arms:
+    # Each repeat starts one arm further on, so that no arm always runs right after the same neighbour: on an H100 held to
+    # 400 W the arm that followed the copy ran up to 30 % slower than in its other repeats.
+    order = args.arms[rep % len(args.arms):] + args.arms[:rep % len(args.arms)]
+    for arm in order:
         with K.config.override(**parse(arm)):
             res[arm].append(timed(arm))
+    print(f"repeat {rep}: " + ", ".join(f"{arm} {res[arm][-1]:.3f}" for arm in order), flush=True)
 gb = 24.0 * B * 1080 * 1920 / 1e6  # bytes the launch must move (read 12 + write 12 per pixel), in MB -> MB / ms = GB / s
 print(f"B={B}, {args.reps} interleaved repeats of {args.steps} launches; min / median / max kernel ms, GB/s at the min:", flush=True)
 for arm in args.arms:

@@ -120,3 +120,5 @@ inline T __shfl_sync(unsigned, T v, int src, int = 32) {
 int atomicAdd(int*, int);
 float atomicAdd(float*, float);
 double atomicAdd(double*, double);
+int atomicMax(int*, int);
+inline int __ffs(int x) { return __builtin_ffs(x); }

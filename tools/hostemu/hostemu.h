@@ -277,6 +277,11 @@ double atomicAdd(double* p, double v) {
   *p = old + v;
   return old;
 }
+int atomicMax(int* p, int v) {
+  const int old = *p;
+  *p = std::max(old, v);
+  return old;
+}
 namespace kb200 {
 namespace tma {
 void emu_spin() {

@@ -390,6 +390,34 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
       compare("warp_fwd_tma<DYN> chunk=" + std::to_string(chunk) + " vs the static deal " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) +
                   " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"), o3, o2, no);
     }
+    // the sweep: every run drawn in raster order (static_pct 0), runs of 1, 2 and 3 tiles; then the same launch restricted to the
+    // footprint class of the wide tile (the producer skips the other class's samples and moves the counter past their runs)
+    // against the static deal restricted the same way, with the rotated sample moved to the front twice so that two
+    // consecutive samples are skipped
+    std::vector<float> o4s, m2(m);
+    float* o4 = aligned(o4s, no);
+    if (B >= 3) {
+      memcpy(&m2[0], &m[18], 9 * sizeof(float));
+      memcpy(&m2[9], &m[18], 9 * sizeof(float));
+      memcpy(&m2[18], &m[0], 9 * sizeof(float));
+    }
+    for (int run : {1, 2, 3}) {
+      const std::string tag = " " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager");
+      for (size_t i = 0; i < no; ++i) o3[i] = -5.f;
+      int counter = 0;
+      TmaWarpParams q = p;
+      q.out = o3; q.counter = &counter; q.chunk_tiles = run; q.static_pct = 0;
+      emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2, true>(map, q); });
+      compare("warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " vs its exact path" + tag, o3, o2, no);
+      for (size_t i = 0; i < no; ++i) o3[i] = o4[i] = -5.f;
+      counter = 0;
+      q.only_class = CLASS_WIDE; q.m = m2.data();
+      emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2, true>(map, q); });
+      TmaWarpParams r = p;
+      r.out = o4; r.only_class = CLASS_WIDE; r.m = m2.data();
+      emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2>(map, r); });
+      compare("warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " wide class only vs the static deal" + tag, o3, o4, no);
+    }
   }
   compare(std::string("warp_fwd_tma (headline, verified on hw) vs its exact path ") + (PROJ ? "projective " : "affine ") + "interp=" + std::to_string(INTERP) + " pad=" + std::to_string(PAD) + " tile " +
               std::to_string(TW) + "x" + std::to_string(TH) + " " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) + " -> " + std::to_string(h) +
