@@ -20,7 +20,9 @@ _PATCHED = {}
 
 def install(kornia_module=None) -> None:
     """Rebind the hot-path functions (and the four callers that have a fused kernel of their own here:
-    ``get_perspective_transform``, ``spatial_gradient``, ``sobel``, ``ssim``) on an imported ``kornia`` package.
+    ``get_perspective_transform``, ``spatial_gradient``, ``sobel``, ``ssim``, plus ``motion_blur`` and
+    ``get_motion_kernel2d``, whose kernel must be built on the GPU) on an imported ``kornia`` package.  A defining
+    module the package lacks is skipped.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -46,10 +48,19 @@ def install(kornia_module=None) -> None:
         "spatial_gradient": ("filters.sobel", filters.spatial_gradient),
         "sobel": ("filters.sobel", filters.sobel),
         "ssim": ("metrics.ssim", metrics.ssim),
+        # motion blur builds its kernel before filter2d sees the image, with rotate on the CPU for number arguments:
+        # both halves are rebound so the reference's MotionBlur / RandomMotionBlur build it on the GPU
+        "motion_blur": ("filters.motion", filters.motion_blur),
+        "get_motion_kernel2d": ("filters.kernels_geometry", filters.get_motion_kernel2d),
     }
     originals = {}
     for name, (mod, fn) in defining.items():
-        m = importlib.import_module(prefix + mod)
+        try:
+            m = importlib.import_module(prefix + mod)
+        except ModuleNotFoundError as e:  # a package without that module (an older kornia): nothing to rebind
+            if e.name is not None and (prefix + mod).startswith(e.name):
+                continue
+            raise
         originals[name] = (_PATCHED.get((m, name), getattr(m, name)), fn)
     for modname, m in list(sys.modules.items()):
         if m is None or not (modname == k.__name__ or modname.startswith(prefix)):

@@ -1,8 +1,9 @@
-"""The three augmentation callers of the hot path (SURVEY.md section 8f row 1), as classes with the reference's constructors:
+"""The augmentation callers of the hot path (SURVEY.md section 8f row 1), as classes with the reference's constructors:
 
     RandomPerspective   kornia/augmentation/_2d/geometric/perspective.py:34-134   -> get_perspective_transform + warp_perspective
     RandomAffine        kornia/augmentation/_2d/geometric/affine.py:33-166        -> get_affine_matrix2d + warp_affine
     RandomGaussianBlur  kornia/augmentation/_2d/intensity/gaussian_blur.py:30-122 -> gaussian_blur2d with per-sample sigmas
+    RandomMotionBlur    kornia/augmentation/_2d/intensity/motion_blur.py          -> motion_blur with per-sample angles / directions
 
 What is kept from the reference's framework (kornia/augmentation/base.py:159-330, _2d/base.py:55-140) is the contract those
 classes expose: ``forward(input, params=None)`` accepting (H,W), (C,H,W) or (B,C,H,W); the parameter dictionaries (same keys,
@@ -25,11 +26,11 @@ import torch
 from torch import nn
 from torch.distributions import Uniform
 
-from .filters import gaussian_blur2d
+from .filters import gaussian_blur2d, motion_blur
 from .geometry._prelude import affine_to_homography
 from .geometry.transform import get_perspective_transform, get_rotation_matrix2d, warp_affine, warp_perspective
 
-__all__ = ["RandomPerspective", "RandomAffine", "RandomGaussianBlur", "get_affine_matrix2d", "get_shear_matrix2d"]
+__all__ = ["RandomPerspective", "RandomAffine", "RandomGaussianBlur", "RandomMotionBlur", "get_affine_matrix2d", "get_shear_matrix2d"]
 
 _RESAMPLE = {0: "nearest", 1: "bilinear", 2: "bicubic", "nearest": "nearest", "bilinear": "bilinear", "bicubic": "bicubic"}
 _PADDING = {0: "zeros", 1: "border", 2: "reflection", 3: "fill", "zeros": "zeros", "border": "border", "reflection": "reflection", "fill": "fill"}
@@ -336,3 +337,67 @@ class RandomGaussianBlur(_RandomAugmentation2D):
         if self.same_on_batch:
             sigma = sigma[:1]
         return gaussian_blur2d(input, kernel_size=flags["kernel_size"], sigma=sigma, border_type=flags["border_type"], separable=flags["separable"])
+
+
+_BORDER = {0: "constant", 1: "reflect", 2: "replicate", 3: "circular", "constant": "constant", "reflect": "reflect", "replicate": "replicate",
+           "circular": "circular"}
+
+
+class RandomMotionBlur(_RandomAugmentation2D):
+    """Motion blur with an angle and a direction drawn per sample and one kernel size for the batch.  Constructor of
+    kornia/augmentation/_2d/intensity/motion_blur.py: ``kernel_size`` an odd int or a (min, max) range, ``angle`` in
+    degrees and ``direction`` in [-1, 1] as a number (the range -x .. x) or a pair."""
+
+    def __init__(self, kernel_size: Union[int, Tuple[int, int]], angle: Union[torch.Tensor, float, Tuple[float, float]],
+                 direction: Union[torch.Tensor, float, Tuple[float, float]], border_type: Union[int, str] = "CONSTANT",
+                 resample: Union[str, int] = "NEAREST", same_on_batch: bool = False, p: float = 0.5, keepdim: bool = False) -> None:
+        super().__init__(p=p, same_on_batch=same_on_batch, keepdim=keepdim)
+        self.kernel_size, self.angle, self.direction = kernel_size, angle, direction
+        # the reference validates when its generator builds the samplers, in the constructor: angle, direction, kernel size
+        _range(angle, "angle", 0.0, (-360, 360))
+        _range(direction, "direction", 0.0, (-1, 1))
+        self._ksize_range()
+        self.flags = {"border_type": _name(_BORDER, border_type, "border_type"), "resample": _name(_RESAMPLE, resample, "resample")}
+
+    def _ksize_range(self) -> Tuple[int, int]:
+        """random_generator/_2d/motion_blur.py make_samplers: the half sizes k // 2 the sampler draws between."""
+        k = self.kernel_size
+        if isinstance(k, int):
+            if not (k >= 3 and k % 2 == 1):
+                raise AssertionError(f"`kernel_size` must be odd and greater than 3. Got {k}.")
+            return k // 2, k // 2
+        if isinstance(k, tuple):
+            if len(k) != 2:
+                raise AssertionError(f"`kernel_size` must be (2,) if it is a tuple. Got {k}.")
+            return k[0] // 2, k[1] // 2
+        raise TypeError(f"Unsupported type: {type(k)}")
+
+    def generate_parameters(self, batch_shape):
+        """MotionBlurGenerator.forward (angle, direction, then kernel size: a CPU draw, since the reference's sampler is
+        built from Python numbers), then RandomMotionBlur.generate_parameters' ``idx``.  The factors land where the
+        reference puts them: on the device and dtype of tensor ``angle`` / ``direction``, else on the CPU in the default
+        dtype."""
+        B, same = batch_shape[0], self.same_on_batch
+        angle = _range(self.angle, "angle", 0.0, (-360, 360))
+        direction = _range(self.direction, "direction", 0.0, (-1, 1))
+        lo, hi = self._ksize_range()
+        angle_factor = _rsample((B,), self._uniform(angle[0], angle[1]), same)
+        direction_factor = _rsample((B,), self._uniform(direction[0], direction[1]), same)
+        ksize_sampler = Uniform(torch.as_tensor(float(lo)), torch.as_tensor(float(hi)), validate_args=False)
+        ksize_factor = _rsample((B,), ksize_sampler, same).int() * 2 + 1
+        dev, dt = torch.empty(0).device, torch.get_default_dtype()
+        for t in (self.angle, self.direction):
+            if isinstance(t, torch.Tensor):
+                dev, dt = t.device, t.dtype
+                break
+        idx = torch.tensor([0]) if B == 0 else torch.randint(B, (1,))
+        return {"ksize_factor": ksize_factor.to(device=dev, dtype=torch.int32), "angle_factor": angle_factor.to(device=dev, dtype=dt),
+                "direction_factor": direction_factor.to(device=dev, dtype=dt), "idx": idx}
+
+    def apply_transform(self, input, params, flags, transform=None):
+        if isinstance(self.kernel_size, int):
+            kernel_size = self.kernel_size
+        else:  # one size for the batch: the one the drawn index picks
+            kernel_size = int(params["ksize_factor"].tolist()[int(params["idx"][0])])
+        return motion_blur(input, kernel_size=kernel_size, angle=params["angle_factor"], direction=params["direction_factor"],
+                           border_type=flags["border_type"], mode=flags["resample"])

@@ -10,6 +10,7 @@
 #include "warp_bwd_tma.cuh"
 #include "sepfilter_tiled.cuh"
 #include "filter2d_tiled.cuh"
+#include "filter2d_taps.cuh"
 #include "remap_tiled.cuh"
 #include "gradient.cuh"
 #include "ssim_vwalk.cuh"
@@ -406,7 +407,9 @@ int kb200_filter2d_forward(const void* x, const void* kernel, void* out, int B, 
   KB_CHECK_ARG((long long)B * C <= MAX_Z, "B*C = %lld planes exceed the %d-plane launch limit", (long long)B * C, MAX_Z);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == KB200_F32) {
-    rc = filter2d_tiled_forward((const float*)x, (const float*)kernel, (float*)out, B, C, H, W, Bk, kh, kw, border, same, st);
+    rc = filter2d_tiled_forward((const float*)x, (const float*)kernel, (float*)out, B, C, H, W, Bk, kh, kw, border, same, st);  // K in {3, 5, 7}
+    if (rc != KB200_EUNSUPPORTED) return rc;
+    rc = filter2d_taps_forward((const float*)x, (const float*)kernel, (float*)out, B, C, H, W, Bk, kh, kw, border, same, st);  // odd K 9..31
     if (rc != KB200_EUNSUPPORTED) return rc;
     return filter2d_forward_t<float>(x, kernel, out, B, C, H, W, Bk, kh, kw, border, same, st);
   }

@@ -43,6 +43,7 @@ using std::min;
 
 // ---- block-level primitives implemented by the scheduler (hostemu.h)
 void __syncthreads();
+int __syncthreads_or(int pred);
 
 // ---- arithmetic intrinsics: compile with -ffp-contract=off so that plain a * b + c is never fused
 inline float __fmaf_rn(float a, float b, float c) { return fmaf(a, b, c); }
@@ -63,6 +64,12 @@ inline int __float_as_int(float f) {
   memcpy(&i, &f, 4);
   return i;
 }
+inline float __int_as_float(int i) {
+  float f;
+  memcpy(&f, &i, 4);
+  return f;
+}
+inline int __popc(unsigned x) { return __builtin_popcount(x); }
 inline float __uint_as_float(unsigned u) {
   float f;
   memcpy(&f, &u, 4);

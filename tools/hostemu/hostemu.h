@@ -29,6 +29,7 @@ struct Fiber {
   std::vector<char> stack;
   bool done = false, at_barrier = false, spinning = false, at_wsync = false;
   unsigned wgen = 0;  // warp collectives completed by this lane
+  unsigned bgen = 0;  // __syncthreads_or barriers passed by this thread
   unsigned lin = 0;   // linear thread index
   uint3 tid;
   std::vector<struct PendingReduce> reduces;  // bulk async-groups are per thread
@@ -56,6 +57,7 @@ static std::deque<PendingTma> pending;
 static std::map<uint64_t*, long long> bar_tx;
 static long long n_tma = 0, n_barriers = 0, n_wsync = 0, n_reduce = 0;
 static std::vector<WarpState> warps;
+static int bar_or[3];  // __syncthreads_or: the votes of generation g go to slot g % 3 (see __syncthreads_or)
 static char* smem_base = nullptr;   // the CTA's shared array (set_smem) for 32-bit shared addresses
 static size_t smem_size = 0;
 static void set_smem(void* base, size_t size) {
@@ -102,13 +104,14 @@ static void run_cta(dim3 block, const std::function<void()>& fn) {
   body = fn;
   blockDim = block;
   warps.assign((n + 31) / 32, WarpState{});
+  bar_or[0] = bar_or[1] = bar_or[2] = 0;
   pending.clear();
   bar_tx.clear();
   for (unsigned i = 0; i < n; ++i) {
     Fiber& f = fibers[i];
     if (f.stack.empty()) f.stack.resize(512 * 1024);
     f.done = f.at_barrier = f.spinning = f.at_wsync = false;
-    f.wgen = 0;
+    f.wgen = f.bgen = 0;
     f.lin = i;
     f.reduces.clear();
     f.tid = make_uint3(i % block.x, (i / block.x) % block.y, i / (block.x * block.y));
@@ -222,6 +225,18 @@ static CUtensorMap make_map(const float* base, int W, int H, int planes, int bw,
 void __syncthreads() {
   emu::cur->at_barrier = true;
   emu::yield();
+}
+// Vote, barrier, read the votes of this generation.  A thread clears the slot of generation g - 1 after barrier g: every
+// thread read it before arriving at g, and generation g + 2, the next to write that slot, starts after barrier g + 1,
+// which this thread has not reached yet.
+int __syncthreads_or(int pred) {
+  emu::Fiber* f = emu::cur;
+  const unsigned g = f->bgen++;
+  if (pred) emu::bar_or[g % 3] = 1;
+  __syncthreads();
+  const int any = emu::bar_or[g % 3];
+  emu::bar_or[(g + 2) % 3] = 0;
+  return any;
 }
 int emu_lane() { return (int)(emu::cur->lin & 31u); }
 unsigned long long emu_warp_exchange(unsigned long long mine, int src_lane) {

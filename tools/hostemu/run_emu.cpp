@@ -11,6 +11,7 @@
 #include "hostemu.h"
 
 #include "../../kornia_b200/csrc/filter2d_tiled.cuh"
+#include "../../kornia_b200/csrc/filter2d_taps.cuh"
 #include "../../kornia_b200/csrc/gradient_tiled.cuh"
 #include "../../kornia_b200/csrc/ssim_vwalk.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
@@ -24,6 +25,7 @@
 namespace kb200 {
 alignas(128) unsigned char sept_smem[256 * 1024];
 alignas(128) unsigned char f2d_smem[256 * 1024];
+alignas(128) unsigned char f2dt_smem[128 * 1024];
 alignas(128) unsigned char gradt_smem[256 * 1024];
 alignas(128) unsigned char ssimv_smem[256 * 1024];
 alignas(128) float ssim_smem[64 * 1024];
@@ -197,6 +199,107 @@ static void test_filter2d(int planes, int H, int W, unsigned grid, bool lazy) {
   compare("filter2d_tiled_kernel (verified on hw) K=" + std::to_string(K) + " border=" + std::to_string(BORDER) + " " + std::to_string(planes) + "x" +
               std::to_string(H) + "x" + std::to_string(W) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
           o, want.data(), want.size());
+}
+
+// ------------------------------------------------------------------------------------------ filter2d, zero-skipping (K 9..31)
+static int emu_strict_failures = 0;
+static void compare_bits(const std::string& what, const float* got, const float* want, size_t n) {  // -0 != +0 here
+  size_t bad = 0, first = 0;
+  for (size_t i = 0; i < n; ++i)
+    if (memcmp(got + i, want + i, 4) != 0) {
+      if (!bad) first = i;
+      ++bad;
+    }
+  if (bad) {
+    printf("FAIL %-72s %zu / %zu differ in their bits, first at %zu: got %.9g want %.9g\n", what.c_str(), bad, n, first, got[first], want[first]);
+    ++failures;
+    ++emu_strict_failures;
+  } else {
+    printf("ok   %s\n", what.c_str());
+  }
+}
+
+// kind 0: a nearest-rotated line (K .. 1.4 K taps), 1: a bilinear-rotated line (~3 K taps), 2: dense, 3: a line with
+// subnormal weights, 4: no nonzero tap at all.  Zero taps are a mix of +0 and -0.
+static void make_taps(float* k, int K, int kind) {
+  std::uniform_real_distribution<float> u(0.05f, 1.f);
+  for (int t = 0; t < K * K; ++t) k[t] = (rng() & 1) ? 0.f : -0.f;
+  if (kind == 4) return;
+  if (kind == 2) {
+    for (int t = 0; t < K * K; ++t) k[t] = u(rng) - 0.5f;
+    return;
+  }
+  const float a = std::uniform_real_distribution<float>(0.f, 3.14159265f)(rng);
+  const float c = (K - 1) * 0.5f, dx = cosf(a), dy = sinf(a);
+  for (int s = 0; s < 4 * K; ++s) {
+    const float r = -c + (2.f * c) * s / (4 * K - 1);
+    const float fx = c + r * dx, fy = c + r * dy;
+    if (kind == 1) {
+      const int x0 = (int)floorf(fx), y0 = (int)floorf(fy);
+      for (int dyy = 0; dyy < 2; ++dyy)
+        for (int dxx = 0; dxx < 2; ++dxx)
+          if (x0 + dxx < K && y0 + dyy < K) k[(y0 + dyy) * K + x0 + dxx] = u(rng) / K;
+    } else {
+      k[(int)lrintf(fy) * K + (int)lrintf(fx)] = kind == 3 ? 1e-41f : u(rng) / K;
+    }
+  }
+}
+
+// specials: 0 none; 1 NaN / +-Inf / -0 / subnormal texels in a few places; 2 tiny texels whose products with the taps
+// underflow (the case where a skipped fma(0, v, -0) would show); 3 every texel -0.
+template <int BORDER>
+static void test_taps(int K, int B, int C, int H, int W, int Bk, int kind, int specials, unsigned grid, bool lazy) {
+  emu::lazy_tma = lazy;
+  const int planes = B * C;
+  std::vector<float> xs, os, ks((size_t)Bk * K * K);
+  float* x = aligned(xs, (size_t)planes * H * W);
+  std::uniform_real_distribution<float> u(-1.f, 1.f);
+  for (size_t i = 0; i < (size_t)planes * H * W; ++i) x[i] = specials == 3 ? -0.f : specials == 2 ? u(rng) * 1e-30f : u(rng);
+  if (specials == 1) {
+    const float sp[6] = {NAN, INFINITY, -INFINITY, -0.f, 1e-40f, -3e-39f};
+    for (int s = 0; s < 12; ++s) x[(size_t)(rng() % ((size_t)planes * H * W))] = sp[s % 6];
+  }
+  for (int b = 0; b < Bk; ++b) make_taps(ks.data() + (size_t)b * K * K, K, kind == 5 ? b % 5 : kind);
+  std::vector<float> want((size_t)planes * H * W);
+  const int h = (K - 1) / 2;
+  for (int pl = 0; pl < planes; ++pl) {
+    const float* kp = ks.data() + (size_t)((pl / C) % Bk) * K * K;
+    for (int y = 0; y < H; ++y)
+      for (int xx = 0; xx < W; ++xx) {
+        float a = 0.f;
+        for (int i = 0; i < K; ++i)
+          for (int j = 0; j < K; ++j) {
+            const int sy = fold(y + i - h, H, BORDER), sx = fold(xx + j - h, W, BORDER);
+            a = fmaf(kp[i * K + j], (sy < 0 || sx < 0) ? 0.f : x[(size_t)pl * H * W + (size_t)sy * W + sx], a);
+          }
+        want[((size_t)pl * H + y) * W + xx] = a;
+      }
+  }
+  float* o = aligned(os, want.size());
+  for (size_t i = 0; i < want.size(); ++i) o[i] = NAN;
+  const CUtensorMap map = emu::make_map(x, W, H, planes, F2DT_BW, SEPT_TH + K - 1, 1);
+  F2dTapsParams p{ks.data(), o, C, H, W, Bk, planes, K};
+  emu::set_smem(f2dt_smem, sizeof(f2dt_smem));
+  if (f2d_taps_smem_bytes(K) > sizeof(f2dt_smem)) emu::fail("filter2d_taps_kernel: shared memory of the CTA exceeds the emulated array");
+  emu::launch(grid, dim3(256), [&] { filter2d_taps_kernel<BORDER>(map, p); });
+  compare_bits("filter2d_taps_kernel vs the dense loop K=" + std::to_string(K) + " border=" + std::to_string(BORDER) + " " + std::to_string(B) + "x" +
+                   std::to_string(C) + "x" + std::to_string(H) + "x" + std::to_string(W) + " Bk=" + std::to_string(Bk) + " kind=" + std::to_string(kind) +
+                   " specials=" + std::to_string(specials) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
+               o, want.data(), want.size());
+}
+
+// The fixed list (also alone: run_emu --taps).  Kernel kinds 0 nearest line, 1 bilinear line, 2 dense, 3 subnormal taps,
+// 4 all zero, 5 one of each per sample; Bk 1, B and cycling; grids that do not divide the strips; special texels.
+static void test_taps_all(bool lazy) {
+  test_taps<KB200_CONSTANT>(9, 2, 3, 70, 132, 2, 0, 0, 5, lazy);
+  test_taps<KB200_REFLECT>(15, 3, 1, 97, 260, 1, 1, 1, 4, lazy);
+  test_taps<KB200_REPLICATE>(31, 3, 2, 40, 136, 2, 5, 1, 3, lazy);
+  test_taps<KB200_REFLECT>(31, 1, 1, 16, 20, 1, 2, 2, 1, lazy);
+  test_taps<KB200_CONSTANT>(15, 2, 1, 33, 8, 2, 3, 0, 2, lazy);
+  test_taps<KB200_REPLICATE>(9, 1, 2, 35, 64, 1, 4, 3, 2, lazy);
+  test_taps<KB200_CONSTANT>(21, 4, 1, 50, 100, 3, 5, 2, 3, lazy);
+  test_taps<KB200_REFLECT>(9, 5, 1, 64, 256, 5, 0, 1, 7, lazy);
+  test_taps<KB200_REFLECT>(15, 2, 1, 40, 64, 2, 3, 2, 3, lazy);  // products that underflow: acc = -0 before a zero tap
 }
 
 template <int K, int NOUT, bool MAG>
@@ -787,7 +890,19 @@ static void fuzz(int rounds) {
   for (int r = 0; r < rounds; ++r) {
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
-    switch (pick(0, 40)) {
+    switch (pick(0, 43)) {
+      case 41:
+      case 42:
+      case 43: {  // zero-skipping filter2d: any odd K 9..31, kernel kind, special texels, Bk 1 / B / cycling
+        const int K = 2 * pick(4, 15) + 1, B = pick(1, 4), C = pick(1, 2), kind = pick(0, 5), specials = pick(0, 3);
+        const int Bk = pick(0, 2) == 0 ? 1 : pick(0, 1) ? B : pick(1, 3);
+        const int h = (K - 1) / 2;
+        const int Hh = std::max(H, h + 1), Wh = std::max(W, 4 * ((h + 4) / 4));
+        if (g() % 3 == 0) test_taps<KB200_CONSTANT>(K, B, C, H, W, Bk, kind, specials, grid, lazy);
+        else if (g() % 2) test_taps<KB200_REFLECT>(K, B, C, Hh, Wh, Bk, kind, specials, grid, lazy);
+        else test_taps<KB200_REPLICATE>(K, B, C, Hh, Wh, Bk, kind, specials, grid, lazy);
+        break;
+      }
       case 35: if (H > 1) test_forward<true, KB200_BORDER, 64, 32, 72, 40, KB200_BICUBIC, false>(3, H, W, std::max(1, H - pick(0, 5)), std::max(4, W - 4 * pick(0, 3)), grid, lazy, pick(0, 1)); break;
       case 36: if (H > 1) test_forward<true, KB200_REFLECTION, 64, 32, 72, 40, KB200_BICUBIC, true>(3, H, W, H, W, grid, lazy, pick(0, 1)); break;
       case 37: if (H > 1) test_forward<false, KB200_REFLECTION, 64, 32, 72, 40, KB200_BICUBIC, false>(3, H, W, std::max(1, H - pick(0, 5)), W, grid, lazy, pick(0, 1)); break;
@@ -840,6 +955,11 @@ int main(int argc, char** argv) {
     probe_forward<KB200_FILL, KB200_BICUBIC>();
     return 0;
   }
+  if (argc == 2 && std::string(argv[1]) == "--taps") {
+    for (int lazy = 0; lazy < 2; ++lazy) test_taps_all(lazy);
+    printf("%s: %d failing comparisons (filter2d_taps_kernel, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
   if (argc == 3 && std::string(argv[1]) == "--fuzz") {
     fuzz(atoi(argv[2]));
     printf("tiles of the forward kernel served by the INNER ('reflection', inside the image) copy of the unit code: %lld of %lld\n", emu_inner_tiles,
@@ -857,6 +977,7 @@ int main(int argc, char** argv) {
     test_sepfilter<5, KB200_REPLICATE>(1, 1, 6, 8, 1, lazy);
     test_sepfilter<17, KB200_REFLECT>(1, 2, 130, 140, 3, lazy);
     test_sepfilter<17, KB200_CONSTANT>(1, 1, 64, 388, 7, lazy);
+    test_taps_all(lazy);
     test_pyrdown<KB200_REFLECT>(3, 70, 132, 4, lazy);
     test_pyrdown<KB200_REPLICATE>(2, 34, 260, 3, lazy);
     test_pyrdown<KB200_CONSTANT>(1, 4, 4, 1, lazy);
