@@ -232,6 +232,23 @@ int kb200_ssim_forward(const void* img1, const void* img2, const void* taps, voi
                        double C1, double C2, double eps, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Feature responses (feature/responses.py:39-282) in ONE kernel each: 4 B read + 4 B written per element.
+ *   x        (planes,H,W) device, planes = B*C
+ *   stencil  HOST pointer to nout*ks*ks doubles exact in fp32: (dx, dy) 3x3 for Harris / GFTT, (dxx, dxy, dyy) ks x ks
+ *            for the Hessian (the taps of spatial_gradient, replicate border)
+ *   blur_taps (blur_k,) device Gaussian taps of the structure-tensor blur (reflect border; Harris / GFTT only, else ignored)
+ *   k        Harris k, rounded to fp32; k_ptr (device fp32) overrides it when not null
+ *   s4       (planes / C,) device fp32 sigmas^4 multiplying each sample's response, or null
+ *   out      (planes,H,W): kind 0 Harris det(M) - k tr(M)^2, kind 1 GFTT min(eig(M)), kind 2 Hessian dxx dyy - dxy^2
+ * One rounding per reference op: bit-identical to the reference's composition over kb200_spatial_gradient_forward and
+ * kb200_sepfilter_forward.  fp32 with W % 4 == 0, 3x3 stencils and blur_k = 7 (Harris, GFTT) or 3x3 / 5x5 stencils
+ * (Hessian) only: anything else returns KB200_EUNSUPPORTED and the host composes the response.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_feature_response_forward(const void* x, const double* stencil, const void* blur_taps, double k, const void* k_ptr,
+                                   const void* s4, void* out, int planes, int C, int H, int W, int stencil_k, int blur_k,
+                                   int kind, int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

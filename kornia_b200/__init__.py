@@ -9,7 +9,7 @@ no CPU path and no fallback -- a missing library or a CPU tensor raises.
 """
 from __future__ import annotations
 
-from . import augmentation, config, core, filters, geometry, graphs, losses, metrics, streaming
+from . import augmentation, config, core, feature, filters, geometry, graphs, losses, metrics, streaming
 from .filters import filter2d, filter2d_separable, gaussian_blur2d
 from .geometry.transform import remap, warp_affine, warp_perspective
 
@@ -21,7 +21,8 @@ _PATCHED = {}
 def install(kornia_module=None) -> None:
     """Rebind the hot-path functions (and the four callers that have a fused kernel of their own here:
     ``get_perspective_transform``, ``spatial_gradient``, ``sobel``, ``ssim``, plus ``motion_blur`` and
-    ``get_motion_kernel2d``, whose kernel must be built on the GPU) on an imported ``kornia`` package.  A defining
+    ``get_motion_kernel2d``, whose kernel must be built on the GPU, and the ``harris_response`` / ``gftt_response`` /
+    ``hessian_response`` of the classical detectors) on an imported ``kornia`` package.  A defining
     module the package lacks is skipped.
 
     Every module of the package that holds a reference to one of the originals is patched: the
@@ -52,6 +53,10 @@ def install(kornia_module=None) -> None:
         # both halves are rebound so the reference's MotionBlur / RandomMotionBlur build it on the GPU
         "motion_blur": ("filters.motion", filters.motion_blur),
         "get_motion_kernel2d": ("filters.kernels_geometry", filters.get_motion_kernel2d),
+        # the modules CornerHarris / CornerGFTT / BlobHessian (and so ScaleSpaceDetector) call these by their global names
+        "harris_response": ("feature.responses", feature.harris_response),
+        "gftt_response": ("feature.responses", feature.gftt_response),
+        "hessian_response": ("feature.responses", feature.hessian_response),
     }
     originals = {}
     for name, (mod, fn) in defining.items():
@@ -78,4 +83,4 @@ def uninstall() -> None:
 
 
 __all__ = ["warp_perspective", "warp_affine", "remap", "filter2d", "filter2d_separable", "gaussian_blur2d", "install",
-           "uninstall", "augmentation", "config", "core", "filters", "geometry", "graphs", "losses", "metrics", "streaming"]
+           "uninstall", "augmentation", "config", "core", "feature", "filters", "geometry", "graphs", "losses", "metrics", "streaming"]

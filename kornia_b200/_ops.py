@@ -745,6 +745,29 @@ _define("ssim_fwd", "(Tensor img1, Tensor img2, Tensor kernel, float C1, float C
         "img1")
 
 
+HARRIS, GFTT, HESSIAN = 0, 1, 2  # kind of kb200_feature_response_forward
+
+
+def _feature_response_cuda(x, stencil, stencil_k, blur, k, k_tensor, s4, kind):
+    _require_cuda(x, "input")
+    xc = x.contiguous()
+    B, C, H, W = xc.shape
+    out = torch.empty_like(xc)
+    host_taps = (ctypes.c_double * len(stencil))(*stencil)
+    with torch.cuda.device(x.device), _Timed("feature_response_forward", x):
+        _lib.call("kb200_feature_response_forward", _ptr(xc), host_taps, _ptr(blur), float(k), _ptr(k_tensor), _ptr(s4), _ptr(out), B * C, C, H, W,
+                  stencil_k, 0 if blur is None else blur.shape[-1], kind, _dtype_code(x), _stream(x))
+    _bump()
+    return out
+
+
+_define("feature_response_fwd",
+        "(Tensor x, float[] stencil, int stencil_k, Tensor? blur, float k, Tensor? k_tensor, Tensor? s4, int kind) -> Tensor",
+        _feature_response_cuda,
+        lambda x, stencil, stencil_k, blur, k, k_tensor, s4, kind: (_fake_same_device(x, blur, k_tensor, s4),
+                                                                      torch.empty_like(x, memory_format=torch.contiguous_format))[1])
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -921,5 +944,5 @@ SpatialGradientFunction = _Apply(spatial_gradient)
 OPERATORS: Tuple[str, ...] = (
     "warp_fwd", "warp_bwd", "warp_prelude", "warp_prelude_bwd", "remap_fwd", "remap_bwd", "filter2d_fwd", "filter2d_bwd_input",
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
-    "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points",
+    "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
 )

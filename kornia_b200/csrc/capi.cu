@@ -14,6 +14,8 @@
 #include "remap_tiled.cuh"
 #include "gradient.cuh"
 #include "ssim_vwalk.cuh"
+#include "corner_vwalk.cuh"
+#include "gradient_tiled.cuh"
 
 namespace kb200 {
 
@@ -583,6 +585,31 @@ int kb200_spatial_gradient_backward(const void* gout, const double* taps, void* 
                                     int dtype, void* stream) {
   KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
   return spatial_gradient_backward(gout, taps, gx, planes, H, W, nout, k, dtype, (cudaStream_t)stream);
+}
+
+int kb200_feature_response_forward(const void* x, const double* stencil, const void* blur_taps, double k, const void* k_ptr, const void* s4,
+                                   void* out, int planes, int C, int H, int W, int stencil_k, int blur_k, int kind, int dtype, void* stream) {
+  KB_CHECK_ARG(x && stencil && out, "null pointer argument");
+  KB_CHECK_ARG(kind == RESP_HARRIS || kind == RESP_GFTT || kind == RESP_HESSIAN, "bad response kind %d", kind);
+  KB_CHECK_ARG(planes > 0 && H > 0 && W > 0 && C > 0 && planes % C == 0, "bad sizes planes=%d C=%d H=%d W=%d", planes, C, H, W);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  const bool corner = kind != RESP_HESSIAN;
+  KB_CHECK_ARG(!corner || blur_taps, "null blur taps");
+  KB_CHECK_ARG(!corner || blur_k != CORNER_K || (CORNER_K / 2 < H && CORNER_K / 2 < W), "reflect border of %d needs an image larger than %d x %d",
+               CORNER_K / 2, H, W);
+  if (dtype != KB200_F32 || (corner ? stencil_k != 3 || blur_k != CORNER_K : stencil_k != 3 && stencil_k != 5)) {
+    set_error("the fused response kernels are fp32 only, with 3x3 stencils and a %d-tap blur (Harris, GFTT) or 3x3 / 5x5 stencils (Hessian)",
+              CORNER_K);
+    return KB200_EUNSUPPORTED;
+  }
+  const int rc = corner ? corner_vwalk_forward((const float*)x, stencil, (const float*)blur_taps, (float)k, (const float*)k_ptr, (const float*)s4,
+                                               (float*)out, planes, C, H, W, kind, (cudaStream_t)stream)
+                        : hessian_tiled_forward((const float*)x, stencil, (const float*)s4, (float*)out, planes, C, H, W, stencil_k,
+                                                (cudaStream_t)stream);
+  if (rc == KB200_EUNSUPPORTED)
+    set_error("the fused response kernels need rows that are a multiple of 4 floats (16-byte aligned) and an image larger than the stencil, "
+              "got H=%d W=%d", H, W);
+  return rc;
 }
 
 int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void* kernel_y, void* out, int B, int C, int H, int W,

@@ -3,15 +3,15 @@
 
 namespace kb200 {
 
-template <int K, int NOUT, bool MAG>
+template <int K, int NOUT, GradEpilogue E>
 static int launch_grad_tiled(const CUtensorMap& map, const GradTiledParams& p, cudaStream_t st) {
   constexpr int BH = SEPT_TH + K - 1;
   constexpr size_t smem = (size_t)(2 * BH * SEPT_BW) * 4 + 2 * sizeof(uint64_t);
-  auto kern = grad_tiled_kernel<K, NOUT, MAG>;
+  auto kern = grad_tiled_kernel<K, NOUT, E>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   KB_SET_SMEM_ONCE(configured, kern, smem);
   const long long nstrips = (long long)p.planes * ceil_div(p.H, SEPT_TH);
-  const long long cap = 3ll * sm_count();
+  const long long cap = (long long)grad_tiled_ctas<K, E>() * sm_count();
   const int grid = (int)(nstrips < cap ? nstrips : cap);
   kern<<<grid, 256, smem, st>>>(map, p);
   cudaError_t e = cudaGetLastError();
@@ -22,36 +22,58 @@ static int launch_grad_tiled(const CUtensorMap& map, const GradTiledParams& p, c
   return KB200_OK;
 }
 
-int spatial_gradient_tiled_forward(const float* x, const double* taps, float* out, int planes, int H, int W, int nout, int k, int magnitude,
-                                   double eps, cudaStream_t st) {
-  if (!option(OPT_TILED_GRADIENT) || !option(OPT_TILED_FILTER)) return KB200_EUNSUPPORTED;
-  if (!x || !out || !taps || (k != 3 && k != 5) || nout < 2 || nout > GRAD_MAX_OUT) return KB200_EUNSUPPORTED;
-  if (magnitude && (nout != 2 || k != 3)) return KB200_EUNSUPPORTED;
-  if ((W % 4) != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0 || (reinterpret_cast<uintptr_t>(out) & 15) != 0) return KB200_EUNSUPPORTED;
-  if (H <= k / 2 || W <= k / 2) return KB200_EUNSUPPORTED;
-  if ((long long)planes * ceil_div(H, SEPT_TH) > 0x7fffffffll) return KB200_EUNSUPPORTED;
+// tensor map and parameters shared by every epilogue; false outside the kernel's envelope
+static bool grad_tiled_setup(const float* x, const double* taps, float* out, int planes, int H, int W, int nout, int k, CUtensorMap& map,
+                             GradTiledParams& p) {
+  if ((W % 4) != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0 || (reinterpret_cast<uintptr_t>(out) & 15) != 0) return false;
+  if (H <= k / 2 || W <= k / 2) return false;
+  if ((long long)planes * ceil_div(H, SEPT_TH) > 0x7fffffffll) return false;
   EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
-  CUtensorMap map;
+  if (!encode) return false;
   const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)planes};
   const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
   const cuuint32_t box[3] = {(cuuint32_t)SEPT_BW, (cuuint32_t)(SEPT_TH + k - 1), 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   if (encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return KB200_EUNSUPPORTED;
-  GradTiledParams p;
+    return false;
   p.out = out;
   p.H = H;
   p.W = W;
   p.planes = planes;
-  p.eps = (float)eps;
+  p.eps = 0.f;
   for (int e = 0; e < nout * k * k; ++e) p.taps[e] = (float)taps[e];  // exact: the host built them in fp32
-  if (magnitude) return launch_grad_tiled<3, 2, true>(map, p, st);
-  if (k == 3 && nout == 2) return launch_grad_tiled<3, 2, false>(map, p, st);
-  if (k == 3 && nout == 3) return launch_grad_tiled<3, 3, false>(map, p, st);
-  if (k == 5 && nout == 3) return launch_grad_tiled<5, 3, false>(map, p, st);
+  p.s4 = nullptr;
+  p.C = 1;
+  return true;
+}
+
+int spatial_gradient_tiled_forward(const float* x, const double* taps, float* out, int planes, int H, int W, int nout, int k, int magnitude,
+                                   double eps, cudaStream_t st) {
+  if (!option(OPT_TILED_GRADIENT) || !option(OPT_TILED_FILTER)) return KB200_EUNSUPPORTED;
+  if (!x || !out || !taps || (k != 3 && k != 5) || nout < 2 || nout > GRAD_MAX_OUT) return KB200_EUNSUPPORTED;
+  if (magnitude && (nout != 2 || k != 3)) return KB200_EUNSUPPORTED;
+  CUtensorMap map;
+  GradTiledParams p;
+  if (!grad_tiled_setup(x, taps, out, planes, H, W, nout, k, map, p)) return KB200_EUNSUPPORTED;
+  p.eps = (float)eps;
+  if (magnitude) return launch_grad_tiled<3, 2, GRAD_MAG>(map, p, st);
+  if (k == 3 && nout == 2) return launch_grad_tiled<3, 2, GRAD_PLANES>(map, p, st);
+  if (k == 3 && nout == 3) return launch_grad_tiled<3, 3, GRAD_PLANES>(map, p, st);
+  if (k == 5 && nout == 3) return launch_grad_tiled<5, 3, GRAD_PLANES>(map, p, st);
   return KB200_EUNSUPPORTED;
+}
+
+int hessian_tiled_forward(const float* x, const double* taps, const float* s4, float* out, int planes, int C, int H, int W, int k,
+                          cudaStream_t st) {
+  if (!option(OPT_TILED_GRADIENT) || !option(OPT_TILED_FILTER)) return KB200_EUNSUPPORTED;
+  if (!x || !out || !taps || (k != 3 && k != 5)) return KB200_EUNSUPPORTED;
+  CUtensorMap map;
+  GradTiledParams p;
+  if (!grad_tiled_setup(x, taps, out, planes, H, W, 3, k, map, p)) return KB200_EUNSUPPORTED;
+  p.s4 = s4;
+  p.C = C;
+  return k == 3 ? launch_grad_tiled<3, 3, GRAD_HESS>(map, p, st) : launch_grad_tiled<5, 3, GRAD_HESS>(map, p, st);
 }
 
 }  // namespace kb200

@@ -6,7 +6,9 @@
 // buffered, the replicate border (kornia/filters/sobel.py:66-68: F.pad(..., 'replicate')) is a patch of the box on edge
 // tiles.  A thread produces 4 columns x R rows of every output plane from a (R+K-1)-row register window fed by aligned
 // LDS.128 -- the L1-gather kernel it replaces re-reads every input row K times through L1 with tiny CTAs (measured
-// 50-66 % of the HBM roofline, DESIGN.md 4.5).  MAG fuses sobel's sqrt(gx^2 + gy^2 + eps) (sobel.py:158-167).
+// 50-66 % of the HBM roofline, DESIGN.md 4.5).  The epilogue E writes the NOUT planes (GRAD_PLANES), or fuses sobel's
+// sqrt(gx^2 + gy^2 + eps) (GRAD_MAG, sobel.py:158-167), or hessian_response's dxx*dyy - dxy^2 times the optional sigma^4
+// of the sample (GRAD_HESS, kornia/feature/responses.py:272-280), one rounding per torch op.
 //
 // Selected by the tiled_gradient switch (gradient.cu).
 #pragma once
@@ -15,17 +17,28 @@
 
 namespace kb200 {
 
+enum GradEpilogue { GRAD_PLANES, GRAD_MAG, GRAD_HESS };
+
 struct GradTiledParams {
-  float* out;  // (planes,NOUT,H,W), or (planes,H,W) for the magnitude
+  float* out;  // (planes,NOUT,H,W), or (planes,H,W) for the magnitude and the Hessian response
   int H, W, planes;
   float eps;
   float taps[GRAD_MAX_OUT * GRAD_MAX_K * GRAD_MAX_K];  // [NOUT][K][K]
+  const float* s4;  // GRAD_HESS: (planes / C,) sigmas^4, or null
+  int C;
 };
 
-template <int K, int NOUT, bool MAG>
-__global__ void __launch_bounds__(256, 3) grad_tiled_kernel(const __grid_constant__ CUtensorMap tmap,
+// resident CTAs per SM: three, except the 5x5 Hessian, which needs more than 80 registers to run without spills
+template <int K, GradEpilogue E>
+constexpr int grad_tiled_ctas() {
+  return E == GRAD_HESS && K == 5 ? 2 : 3;
+}
+
+template <int K, int NOUT, GradEpilogue E>
+__global__ void __launch_bounds__(256, grad_tiled_ctas<K, E>()) grad_tiled_kernel(const __grid_constant__ CUtensorMap tmap,
                                                             const __grid_constant__ GradTiledParams p) {
-  static_assert((K == 3 || K == 5) && NOUT >= 2 && NOUT <= GRAD_MAX_OUT && (!MAG || (NOUT == 2 && K == 3)), "stencil limits");
+  static_assert((K == 3 || K == 5) && NOUT >= 2 && NOUT <= GRAD_MAX_OUT && (E != GRAD_MAG || (NOUT == 2 && K == 3)) &&
+                (E != GRAD_HESS || NOUT == 3), "stencil limits");
   constexpr int HALO = (K - 1) / 2;
   constexpr int TW = SEPT_TW, TH = SEPT_TH, BW = SEPT_BW;
   constexpr int BH = TH + K - 1;
@@ -91,7 +104,8 @@ __global__ void __launch_bounds__(256, 3) grad_tiled_kernel(const __grid_constan
   for (int seg = 0; segs.get(seg, strip, tx0, tx1, cursor); ++seg) {
     const int plane = strip / tiles_y, ty = strip - plane * tiles_y;
     const int y0 = ty * TH;
-    float* oplane = p.out + (size_t)plane * (MAG ? 1 : NOUT) * HW;
+    float* oplane = p.out + (size_t)plane * (E == GRAD_PLANES ? NOUT : 1) * HW;
+    const float s4 = E == GRAD_HESS && p.s4 ? __ldg(p.s4 + plane / p.C) : 1.0f;
 
     for (int tx = tx0; tx < tx1; ++tx, ++n) {
       const int s = n & 1;
@@ -153,12 +167,20 @@ __global__ void __launch_bounds__(256, 3) grad_tiled_kernel(const __grid_constan
           for (int r = 0; r < R; ++r) {
             const int gy = y0 + row0 + r;
             if (gy < p.H) {
-              if (MAG) {
+              if (E == GRAD_MAG) {
                 float m[4];
 #pragma unroll
                 for (int x = 0; x < 4; ++x)
                   m[x] = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(acc[0][r][x], acc[0][r][x]), __fmul_rn(acc[1][r][x], acc[1][r][x])), p.eps));
                 __stcs(reinterpret_cast<float4*>(oplane + (size_t)gy * p.W + gx0), make_float4(m[0], m[1], m[2], m[3]));
+              } else if (E == GRAD_HESS) {  // (dxx, dxy, dyy): dxx * dyy - dxy**2, then * sigmas.pow(4)
+                float h[4];
+#pragma unroll
+                for (int x = 0; x < 4; ++x) {
+                  h[x] = __fsub_rn(__fmul_rn(acc[0][r][x], acc[2][r][x]), __fmul_rn(acc[1][r][x], acc[1][r][x]));
+                  if (p.s4) h[x] = __fmul_rn(h[x], s4);
+                }
+                __stcs(reinterpret_cast<float4*>(oplane + (size_t)gy * p.W + gx0), make_float4(h[0], h[1], h[2], h[3]));
               } else {
 #pragma unroll
                 for (int o = 0; o < NOUT; ++o)
@@ -178,5 +200,9 @@ __global__ void __launch_bounds__(256, 3) grad_tiled_kernel(const __grid_constan
 // KB200_EUNSUPPORTED -> the caller runs spatial_gradient_fwd.
 int spatial_gradient_tiled_forward(const float* x, const double* taps, float* out, int planes, int H, int W, int nout, int k, int magnitude,
                                    double eps, cudaStream_t st);
+// hessian_response: taps (3,k,k) = (dxx, dxy, dyy), out (planes,H,W), s4 (planes / C,) or null.  KB200_EUNSUPPORTED -> the caller
+// composes spatial_gradient and torch elementwise ops.
+int hessian_tiled_forward(const float* x, const double* taps, const float* s4, float* out, int planes, int C, int H, int W, int k,
+                          cudaStream_t st);
 
 }  // namespace kb200

@@ -14,6 +14,7 @@
 #include "../../kornia_b200/csrc/filter2d_taps.cuh"
 #include "../../kornia_b200/csrc/gradient_tiled.cuh"
 #include "../../kornia_b200/csrc/ssim_vwalk.cuh"
+#include "../../kornia_b200/csrc/corner_vwalk.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -28,6 +29,7 @@ alignas(128) unsigned char f2d_smem[256 * 1024];
 alignas(128) unsigned char f2dt_smem[128 * 1024];
 alignas(128) unsigned char gradt_smem[256 * 1024];
 alignas(128) unsigned char ssimv_smem[256 * 1024];
+alignas(128) unsigned char corner_smem[256 * 1024];
 alignas(128) float ssim_smem[64 * 1024];
 alignas(128) unsigned char remap_smem[256 * 1024];
 alignas(128) unsigned char tma_smem[256 * 1024];
@@ -326,7 +328,7 @@ static void test_gradient(int planes, int H, int W, unsigned grid, bool lazy) {
   }
   p.out = aligned(os, want.size());
   const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
-  emu::launch(grid, dim3(256), [&] { grad_tiled_kernel<K, NOUT, MAG>(map, p); });
+  emu::launch(grid, dim3(256), [&] { grad_tiled_kernel<K, NOUT, MAG ? GRAD_MAG : GRAD_PLANES>(map, p); });
   compare("grad_tiled_kernel K=" + std::to_string(K) + " NOUT=" + std::to_string(NOUT) + (MAG ? " MAG " : "     ") + std::to_string(planes) + "x" +
               std::to_string(H) + "x" + std::to_string(W) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
           p.out, want.data(), want.size());
@@ -365,6 +367,158 @@ static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy) {
   compare("ssim_vwalk_kernel vs ssim_tiled_kernel " + tag, o2, o1, n);
 }
 
+
+// bits equal (-0 != +0), or NaN on both sides: the device returns one canonical NaN, while on x86 the sign of a NaN produced
+// from two NaN operands depends on which operand the compiler put first in a commutative op
+static void compare_bits_or_nan(const std::string& what, const float* got, const float* want, size_t n) {
+  size_t bad = 0, first = 0;
+  for (size_t i = 0; i < n; ++i)
+    if (memcmp(got + i, want + i, 4) != 0 && !(got[i] != got[i] && want[i] != want[i])) {
+      if (!bad) first = i;
+      ++bad;
+    }
+  if (bad) {
+    printf("FAIL %-72s %zu / %zu differ in their bits, first at %zu: got %.9g want %.9g\n", what.c_str(), bad, n, first, got[first], want[first]);
+    ++failures;
+    ++emu_strict_failures;
+  } else {
+    printf("ok   %s\n", what.c_str());
+  }
+}
+
+// ------------------------------------------------------------------------------------------ feature responses
+// Scalar restatement of kornia/feature/responses.py as this library composes it: spatial_gradient (replicate border,
+// row-major FMA over every tap), the products, gaussian_blur2d's row then column pass (reflect border, ascending FMA),
+// then one rounding per torch op; torch.min propagates NaN; times sigmas^4.  Compared bit for bit (-0 != +0) with
+// corner_vwalk_kernel (Harris, GFTT) and grad_tiled_kernel<GRAD_HESS>.
+static const float kSobel1[18] = {-1 / 8.f, 0, 1 / 8.f, -2 / 8.f, 0, 2 / 8.f, -1 / 8.f, 0, 1 / 8.f,
+                                  -1 / 8.f, -2 / 8.f, -1 / 8.f, 0, 0, 0, 1 / 8.f, 2 / 8.f, 1 / 8.f};
+static const float kDiff1[18] = {0, 0, 0, -0.5f, 0, 0.5f, 0, 0, 0, 0, -0.5f, 0, 0, 0, 0, 0, 0.5f, 0};
+
+static void special_texels(float* x, size_t n, int specials) {
+  if (!specials) return;
+  const float v[8] = {NAN, INFINITY, -INFINITY, -0.f, 1e-40f, -1e-41f, 1e-38f, 3e38f};
+  for (size_t i = 0; i < n; i += 97 + (rng() % 300)) x[i] = v[rng() % 8];
+  x[0] = 1e-40f;
+  x[n - 1] = -0.f;
+}
+
+template <int KIND>
+static void test_corner(int planes, int C, int H, int W, bool diff, int specials, bool sigmas, unsigned grid, bool lazy) {
+  emu::lazy_tma = lazy;
+  const size_t HW = (size_t)H * W, n = (size_t)planes * HW;
+  std::vector<float> xs, os;
+  float* x = aligned(xs, n);
+  for (size_t i = 0; i < n; ++i) x[i] = randv(1)[0];
+  special_texels(x, n, specials);
+  const float* st = diff ? kDiff1 : kSobel1;
+  float g[CORNER_K], gs = 0.f;
+  for (int j = 0; j < CORNER_K; ++j) gs += (g[j] = expf(-0.5f * (float)((j - 3) * (j - 3))));
+  for (int j = 0; j < CORNER_K; ++j) g[j] /= gs;
+  std::vector<float> s4(planes / C);
+  for (auto& v : s4) v = randv(1, 0.5f, 3.f)[0];
+  const float k = 0.04f;
+  std::vector<float> want(n), prod(3 * HW), row(3 * HW);
+  for (int p = 0; p < planes; ++p) {
+    const float* xp = x + p * HW;
+    for (int y = 0; y < H; ++y)
+      for (int xx = 0; xx < W; ++xx) {
+        float d[2] = {0.f, 0.f};
+        for (int o = 0; o < 2; ++o)
+          for (int i = 0; i < 3; ++i)
+            for (int j = 0; j < 3; ++j)
+              d[o] = fmaf(st[(o * 3 + i) * 3 + j], xp[(size_t)fold(y + i - 1, H, KB200_REPLICATE) * W + fold(xx + j - 1, W, KB200_REPLICATE)], d[o]);
+        prod[y * W + xx] = d[0] * d[0];
+        prod[HW + y * W + xx] = d[1] * d[1];
+        prod[2 * HW + y * W + xx] = d[0] * d[1];
+      }
+    for (int q = 0; q < 3; ++q)
+      for (int y = 0; y < H; ++y)
+        for (int xx = 0; xx < W; ++xx) {
+          float a = 0.f;
+          for (int j = 0; j < CORNER_K; ++j) a = fmaf(g[j], prod[q * HW + y * W + fold(xx + j - 3, W, KB200_REFLECT)], a);
+          row[q * HW + y * W + xx] = a;
+        }
+    for (int y = 0; y < H; ++y)
+      for (int xx = 0; xx < W; ++xx) {
+        float m[3];
+        for (int q = 0; q < 3; ++q) {
+          float a = 0.f;
+          for (int i = 0; i < CORNER_K; ++i) a = fmaf(g[i], row[q * HW + (size_t)fold(y + i - 3, H, KB200_REFLECT) * W + xx], a);
+          m[q] = a;
+        }
+        const float det = m[0] * m[1] - m[2] * m[2], tr = m[0] + m[1], tr2 = tr * tr;
+        float r;
+        if (KIND == RESP_HARRIS) {
+          r = det - k * tr2;
+        } else {
+          const float sq = sqrtf(fabsf(tr2 - 4.f * det)), e1 = 0.5f * (tr + sq), e2 = 0.5f * (tr - sq);
+          r = e1 != e1 ? e1 : e2 != e2 ? e2 : fminf(e1, e2);
+        }
+        want[p * HW + y * W + xx] = sigmas ? r * s4[p / C] : r;
+      }
+  }
+  CornerParams prm;
+  prm.taps = g; prm.kptr = nullptr; prm.s4 = sigmas ? s4.data() : nullptr; prm.out = aligned(os, n);
+  prm.planes = planes; prm.C = C; prm.H = H; prm.W = W; prm.k = k;
+  for (int e = 0; e < 18; ++e) prm.st[e] = st[e];
+  const CUtensorMap map = emu::make_map(x, W, H, planes, SSIMV_BW, SSIMV_TH + 2, 1), pro = emu::make_map(x, W, H, planes, SSIMV_BW, CORNER_K - 1 + 2, 1);
+  emu::launch(grid, dim3(256), [&] { corner_vwalk_kernel<KIND>(map, pro, prm); });
+  compare_bits_or_nan(std::string("corner_vwalk_kernel ") + (KIND == RESP_HARRIS ? "Harris" : "GFTT") + (diff ? " diff " : " sobel ") + std::to_string(planes) + "x" +
+                   std::to_string(H) + "x" + std::to_string(W) + " C=" + std::to_string(C) + (sigmas ? " sigmas" : "") + (specials ? " special texels" : "") +
+                   " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
+               prm.out, want.data(), n);
+}
+
+template <int K>
+static void test_hessian(int planes, int C, int H, int W, int specials, bool sigmas, unsigned grid, bool lazy) {
+  emu::lazy_tma = lazy;
+  const size_t HW = (size_t)H * W, n = (size_t)planes * HW;
+  std::vector<float> xs, os;
+  float* x = aligned(xs, n);
+  for (size_t i = 0; i < n; ++i) x[i] = randv(1)[0];
+  special_texels(x, n, specials);
+  GradTiledParams p;
+  p.H = H; p.W = W; p.planes = planes; p.eps = 0.f; p.C = C;
+  auto t = randv(3 * K * K, -1.f, 1.f);
+  for (int e = 0; e < 3 * K * K; ++e) p.taps[e] = (e % 4 == 1) ? 0.f : t[e];
+  std::vector<float> s4(planes / C);
+  for (auto& v : s4) v = randv(1, 0.5f, 3.f)[0];
+  p.s4 = sigmas ? s4.data() : nullptr;
+  std::vector<float> d(3 * n), want(n);
+  ref_filter2d(x, p.taps, 3, d.data(), planes, H, W, K, KB200_REPLICATE);
+  for (int pl = 0; pl < planes; ++pl)
+    for (size_t i = 0; i < HW; ++i) {
+      const float* dp = d.data() + (size_t)pl * 3 * HW;
+      const float h = dp[i] * dp[2 * HW + i] - dp[HW + i] * dp[HW + i];
+      want[pl * HW + i] = sigmas ? h * s4[pl / C] : h;
+    }
+  p.out = aligned(os, n);
+  const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
+  emu::launch(grid, dim3(256), [&] { grad_tiled_kernel<K, 3, GRAD_HESS>(map, p); });
+  compare_bits_or_nan("grad_tiled_kernel<GRAD_HESS> K=" + std::to_string(K) + " " + std::to_string(planes) + "x" + std::to_string(H) + "x" + std::to_string(W) +
+                   " C=" + std::to_string(C) + (sigmas ? " sigmas" : "") + (specials ? " special texels" : "") + " grid=" + std::to_string(grid) +
+                   (lazy ? " lazy" : " eager"),
+               p.out, want.data(), n);
+}
+
+// The fixed list (also alone: run_emu --responses): edge bands (W = 4, 68, 132), H % 32 in {1, 2} (the last tile's box lies
+// entirely below the image), H = W = 4, grids that do not divide the bands (segments that start in the middle of a band),
+// both stencil modes, sigmas, and NaN / +-Inf / -0 / subnormal texels.
+static void test_responses_all(bool lazy) {
+  test_corner<RESP_HARRIS>(3, 3, 70, 132, false, 0, true, 4, lazy);
+  test_corner<RESP_HARRIS>(2, 1, 65, 68, true, 1, false, 3, lazy);
+  test_corner<RESP_HARRIS>(1, 1, 4, 4, false, 1, true, 1, lazy);
+  test_corner<RESP_HARRIS>(2, 2, 97, 200, false, 1, true, 5, lazy);
+  test_corner<RESP_GFTT>(3, 3, 66, 132, false, 1, true, 7, lazy);
+  test_corner<RESP_GFTT>(2, 1, 33, 4, true, 1, false, 2, lazy);
+  test_corner<RESP_GFTT>(1, 1, 34, 68, true, 0, true, 1, lazy);
+  test_corner<RESP_GFTT>(4, 2, 129, 72, false, 1, false, 9, lazy);
+  test_hessian<5>(3, 3, 70, 132, 1, true, 4, lazy);
+  test_hessian<3>(2, 1, 33, 68, 1, false, 3, lazy);
+  test_hessian<5>(1, 1, 4, 4, 0, true, 1, lazy);
+  test_hessian<3>(2, 2, 65, 260, 1, true, 5, lazy);
+}
 
 // ------------------------------------------------------------------------------------------ remap / fused undistort
 static float ref_remap_pixel(const float* plane, int H, int W, float mx, float my) {
@@ -890,7 +1044,19 @@ static void fuzz(int rounds) {
   for (int r = 0; r < rounds; ++r) {
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
-    switch (pick(0, 43)) {
+    switch (pick(0, 46)) {
+      case 44:
+      case 45:
+      case 46: {  // feature responses: Harris / GFTT / Hessian, both stencil modes, C 1..3, sigmas, special texels
+        const int C = pick(1, 3), B = pick(1, 2), specials = pick(0, 1), sig = pick(0, 1), diff = pick(0, 1);
+        const int Hh = std::max(H, 4), Wh = std::max(W, 4);
+        const int which = pick(0, 3);
+        if (which == 0) test_corner<RESP_HARRIS>(B * C, C, Hh, Wh, diff, specials, sig, grid, lazy);
+        else if (which == 1) test_corner<RESP_GFTT>(B * C, C, Hh, Wh, diff, specials, sig, grid, lazy);
+        else if (which == 2) test_hessian<3>(B * C, C, Hh, Wh, specials, sig, grid, lazy);
+        else test_hessian<5>(B * C, C, Hh, Wh, specials, sig, grid, lazy);
+        break;
+      }
       case 41:
       case 42:
       case 43: {  // zero-skipping filter2d: any odd K 9..31, kernel kind, special texels, Bk 1 / B / cycling
@@ -958,6 +1124,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--taps") {
     for (int lazy = 0; lazy < 2; ++lazy) test_taps_all(lazy);
     printf("%s: %d failing comparisons (filter2d_taps_kernel, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--responses") {
+    for (int lazy = 0; lazy < 2; ++lazy) test_responses_all(lazy);
+    printf("%s: %d failing comparisons (feature responses, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 3 && std::string(argv[1]) == "--fuzz") {
