@@ -232,7 +232,9 @@ struct PixelSampler {
       cubic_weights<T>(R::sub(iy, fy), cy);
 #pragma unroll
       for (int i = 0; i < NT; ++i) {
-        const int xi = (int)pad_coord<T, SPAD>(R::add(R::sub(fx, T(1)), T(i)), W, align);
+        // the tap coordinates as ATen's forward spells them: ix_nw - 1, ix_nw + 0, ix_nw + 1, ix_nw + 2 but iy_nw - 1 + i.  The
+        // same values below 2^24; beyond it (fx - 1) + 2 and fx + 1 round differently, which 'reflection' folds to other texels.
+        const int xi = (int)pad_coord<T, SPAD>(R::add(fx, T(i - 1)), W, align);
         const int yi = (int)pad_coord<T, SPAD>(R::add(R::sub(fy, T(1)), T(i)), H, align);
         xok[i] = (unsigned)xi < (unsigned)W;
         yok[i] = (unsigned)yi < (unsigned)H;

@@ -242,10 +242,10 @@ __global__ void __launch_bounds__(BWD_THREADS, 2) warp_bwd_tma2(const __grid_con
           float ix = unnorm<ALIGN>(gx, Wm1, Wf), iy = unnorm<ALIGN>(gy, Hm1, Hf);
           float px = 1.f, py = 1.f;  // d(padded coordinate)/d(coordinate): 0 where the border clamp is active
           if (PAD == KB200_BORDER) {
-            if (!(ix > 0.f && ix < Wm1)) px = 0.f;
-            if (!(iy > 0.f && iy < Hm1)) py = 0.f;
-            ix = fminf(Wm1, fmaxf(ix, 0.f));
-            iy = fminf(Hm1, fmaxf(iy, 0.f));
+            // pad_coord_grad's clamp (ATen's clip_coordinates_set_grad): comparisons, so a NaN coordinate stays NaN, takes the
+            // exact path and scatters nothing -- fminf / fmaxf would turn it into texel 0
+            if (ix <= 0.f) { ix = 0.f; px = 0.f; } else if (ix >= Wm1) { ix = Wm1; px = 0.f; }
+            if (iy <= 0.f) { iy = 0.f; py = 0.f; } else if (iy >= Hm1) { iy = Hm1; py = 0.f; }
           }
           const float tX = __fadd_rd(ix, FLOOR_MAGIC), tY = __fadd_rd(iy, FLOOR_MAGIC);
           const int X = __float_as_int(tX), Y = __float_as_int(tY);

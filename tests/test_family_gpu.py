@@ -234,6 +234,12 @@ def test_fused_unsharp_equals_blur_then_lerp(ks, border):
     torch.testing.assert_close(fused, two_step, rtol=1e-6, atol=1e-6)
     print(f"unsharp k={ks}: {(fused == two_step).float().mean().item() * 100:.2f}% bit-identical to blur + torch.lerp")
     torch.testing.assert_close(fused, R.unsharp_mask(x, (ks, ks), (1.3, 1.7), border), **FP32)
+    from test_nonfinite_gpu import classes_equal, diff, special_image
+
+    xs = special_image(*x.shape, seed=ks)   # NaN / Inf / -0 / subnormal texels: the same classes, the same tolerance
+    fused = K.filters.unsharp_mask(xs, (ks, ks), (1.3, 1.7), border)
+    two_step = torch.lerp(K.filters.gaussian_blur2d(xs, (ks, ks), (1.3, 1.7), border), xs, weight=2.0)
+    assert classes_equal(fused, two_step, rtol=1e-6, atol=1e-6), diff(fused, two_step)
     # outside the fused envelope (non-square kernel, gradient needed): the composition
     torch.testing.assert_close(K.filters.unsharp_mask(x, (3, 5), (1.0, 1.0)), R.unsharp_mask(x, (3, 5), (1.0, 1.0)), **FP32)
     leaf = x.clone().requires_grad_(True)

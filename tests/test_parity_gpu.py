@@ -237,20 +237,19 @@ _TILED_CASES = ([("bilinear", pad, C) for pad in ("zeros", "border", "reflection
 @pytest.mark.parametrize("mode,pad,C", _TILED_CASES)
 @pytest.mark.parametrize("ac", [True, False])
 def test_tiled_kernel_bit_identical_to_generic(mode, pad, C, ac):
-    """Every mode the tiled kernel serves must reproduce the generic kernel exactly (the staged tile is only a
-    cache): rotations, zoom, strong perspective, a horizon inside the image, everything out of view."""
+    """Every mode the tiled kernel serves must reproduce the generic kernel exactly, -0 and NaN included (the staged tile is
+    only a cache): rotations, zoom, strong perspective, a horizon inside the image, everything out of view; on a random image
+    and on one with NaN / Inf / -0 / subnormal texels at the tile seams."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
     H, W = 216, 384
     M = torch.cat([_wild_matrices(H, W), _shift_matrices(W), _bench_homographies(6, H, W, 5, sigma=4.0)]).to(DEV)
-    src = torch.rand(M.shape[0], C, H, W, device=DEV)
     fv = torch.tensor([0.2, 0.5, 0.8], device=DEV) if pad == "fill" else None
     from kornia_b200 import _lib
 
-    def same(a, b):
-        if mode == "nearest":  # identical arithmetic; NaN-safe comparison
-            return torch.equal(a.nan_to_num(nan=-7.0), b.nan_to_num(nan=-7.0))
-        return torch.equal(a.nan_to_num(nan=-7.0), b.nan_to_num(nan=-7.0))
-
-    for dsize in ((H, W), (150, 333)):
+    same = bits_equal
+    for src, dsize in ((torch.rand(M.shape[0], C, H, W, device=DEV), (H, W)), (torch.rand(M.shape[0], C, H, W, device=DEV), (150, 333)),
+                       (special_image(M.shape[0], C, H, W, seed=C), (H, W)), (special_image(M.shape[0], C, H, W, seed=C), (150, 333))):
         a = K.warp_perspective(src, M, dsize, mode=mode, padding_mode=pad, align_corners=ac, fill_value=fv)
         assert _lib.last_warp_variant() == "tma_tile"
         b = _generic(lambda: K.warp_perspective(src, M, dsize, mode=mode, padding_mode=pad, align_corners=ac, fill_value=fv))
@@ -386,7 +385,11 @@ def test_prelude_keeps_autograd_path():
 @pytest.mark.parametrize("border", ["constant", "reflect", "replicate"])
 @pytest.mark.parametrize("k", [3, 5, 7, 9, 11, 13, 15, 17])
 def test_tiled_sepfilter_bit_identical_to_generic(k, border):
-    """Per-sample taps exercise the b % Bk indexing; 37 x 3 x 200 x 520 has more strips than the persistent grid has CTAs."""
+    """Per-sample taps exercise the b % Bk indexing; 37 x 3 x 200 x 520 has more strips than the persistent grid has CTAs.
+    Each shape also runs on an image with NaN / Inf / -0 / subnormal texels at the tile seams (against the generic kernel,
+    bit for bit with -0 != +0; tests/test_nonfinite_gpu.py checks it against the reference)."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
     g = torch.Generator().manual_seed(k)
     shapes = ((2, 3, 70, 200), (1, 1, 32, 128), (3, 2, 45, 132), (1, 3, 9 + k, 12 + 4 * (k // 4)), (3, 2, 33, 4), (1, 1, 6, 8),
               (2, 3, 1080, 1920), (37, 3, 200, 520))
@@ -396,10 +399,12 @@ def test_tiled_sepfilter_bit_identical_to_generic(k, border):
         x = torch.rand(B, C, H, W, generator=g).to(DEV)
         kx = torch.randn(B, k, generator=g).to(DEV)
         ky = torch.randn(1, k, generator=g).to(DEV)
+        for xx in (x, special_image(B, C, H, W, seed=k)) if B * C * H * W < 10 ** 6 else (x,):
+            a = K.filter2d_separable(xx, kx, ky, border)
+            with K.config.override(tiled_filter=0):
+                b = K.filter2d_separable(xx, kx, ky, border)
+            assert bits_equal(a, b), (B, C, H, W, float((a - b).abs().nan_to_num().max()))
         a = K.filter2d_separable(x, kx, ky, border)
-        with K.config.override(tiled_filter=0):
-            b = K.filter2d_separable(x, kx, ky, border)
-        assert torch.equal(a, b), (B, C, H, W, float((a - b).abs().max()))
         want = R.filter2d_separable(x.cpu(), kx.cpu(), ky.cpu(), border)
         torch.testing.assert_close(a.cpu(), want, rtol=1e-4, atol=1e-5)
 
@@ -522,18 +527,23 @@ def test_gradients_match_the_same_device_reference_at_the_cfg4_shape(images):
 @pytest.mark.parametrize("border", ["constant", "reflect", "replicate"])
 @pytest.mark.parametrize("k", [3, 5, 7])
 def test_tiled_filter2d_bit_identical_to_generic(k, border):
-    import os
+    """Also on an image with NaN / Inf / -0 / subnormal texels at the tile seams and a sample of -0 (against the generic kernel
+    only).  The third kernel has only positive taps, like a blur: then a -0 sample filters to -0 or +0 depending on how the
+    accumulator is seeded, which bits_equal sees and torch.equal does not."""
+    from test_nonfinite_gpu import bits_equal, special_image
 
     g = torch.Generator().manual_seed(10 + k)
     for (B, C, H, W) in ((2, 3, 70, 200), (1, 1, 32, 128), (4, 2, 45, 132), (1, 3, 6 + k, 12)):
         x = torch.rand(B, C, H, W, generator=g).to(DEV)
-        for kern in (torch.randn(1, k, k, generator=g), torch.randn(B, k, k, generator=g)):
+        for kern in (torch.randn(1, k, k, generator=g), torch.randn(B, k, k, generator=g), torch.rand(1, k, k, generator=g)):
             kern = kern.to(DEV)
             for normalized, behaviour in ((False, "corr"), (True, "conv")):
+                for xx in (x, special_image(B, C, H, W, seed=k)):
+                    a = K.filter2d(xx, kern, border, normalized=normalized, behaviour=behaviour)
+                    with K.config.override(tiled_filter=0):
+                        b = K.filter2d(xx, kern, border, normalized=normalized, behaviour=behaviour)
+                    assert bits_equal(a, b), (B, C, H, W, float((a - b).abs().nan_to_num().max()))
                 a = K.filter2d(x, kern, border, normalized=normalized, behaviour=behaviour)
-                with K.config.override(tiled_filter=0):
-                    b = K.filter2d(x, kern, border, normalized=normalized, behaviour=behaviour)
-                assert torch.equal(a, b), (B, C, H, W, float((a - b).abs().max()))
                 want = R.filter2d(x.cpu(), kern.cpu(), border, normalized=normalized, behaviour=behaviour)
                 torch.testing.assert_close(a.cpu(), want, rtol=1e-4, atol=1e-5)
 
@@ -542,7 +552,10 @@ def test_tiled_filter2d_bit_identical_to_generic(k, border):
 @pytest.mark.parametrize("ac", [None, True])
 @pytest.mark.parametrize("C", [3, 1])
 def test_tiled_remap_bit_identical_to_generic(pad, ac, C):
-    """Smooth maps (served from the staged box), a noisy map (mostly exact path), out-of-view and NaN entries."""
+    """Smooth maps (served from the staged box), a noisy map (mostly exact path), out-of-view and NaN entries; then special
+    texels under the same maps, and maps with NaN / Inf / beyond-int / -0 / edge entries at the tile seams."""
+    from test_nonfinite_gpu import _special_maps, bits_equal, special_image
+
     H, W, h, w = 96, 160, 80, 136
     g = torch.Generator().manual_seed(4)
     img = torch.rand(3, C, H, W, generator=g).to(DEV)
@@ -556,10 +569,13 @@ def test_tiled_remap_bit_identical_to_generic(pad, ac, C):
     bad_x[::7, ::5] = float("nan")
     mx = torch.stack([smooth_x, noisy_x, bad_x]).to(DEV)
     my = torch.stack([smooth_y, noisy_y, smooth_y]).to(DEV)
-    for (ax, ay) in ((mx, my), (far_x[None].to(DEV), smooth_y[None].to(DEV)), (smooth_x[None].to(DEV), smooth_y[None].to(DEV))):
-        a = K.remap(img, ax, ay, padding_mode=pad, align_corners=ac)
-        b = _generic(lambda: K.remap(img, ax, ay, padding_mode=pad, align_corners=ac), check_variant=False)
-        assert torch.equal(a.nan_to_num(nan=-7.0), b.nan_to_num(nan=-7.0)), float((a - b).abs().nan_to_num().max())
+    sx, sy = _special_maps(H, W, h, w, seed=C)
+    special = special_image(3, C, H, W, seed=C)
+    for (im, ax, ay) in ((img, mx, my), (img, far_x[None].to(DEV), smooth_y[None].to(DEV)), (img, smooth_x[None].to(DEV), smooth_y[None].to(DEV)),
+                         (special, mx, my), (special, sx[None].to(DEV), sy[None].to(DEV))):
+        a = K.remap(im, ax, ay, padding_mode=pad, align_corners=ac)
+        b = _generic(lambda: K.remap(im, ax, ay, padding_mode=pad, align_corners=ac), check_variant=False)
+        assert bits_equal(a, b), float((a - b).abs().nan_to_num().max())
     want = R.remap(img.cpu()[:1], smooth_x[None], smooth_y[None], padding_mode=pad, align_corners=ac)
     got = K.remap(img[:1], smooth_x[None].to(DEV), smooth_y[None].to(DEV), padding_mode=pad, align_corners=ac)
     torch.testing.assert_close(got.cpu(), want, rtol=1e-4, atol=1e-5)

@@ -8,6 +8,7 @@ import torch
 import kornia_b200 as K
 from kornia_b200 import _lib
 from kornia_b200.geometry import _prelude as P
+from test_nonfinite_gpu import bits_equal
 from test_parity_gpu import _bench_homographies, _wild_matrices
 
 pytestmark = pytest.mark.gpu
@@ -57,8 +58,8 @@ def test_sweep_bit_identical_to_strip_deal_and_generic(batch, pad, projective):
             with K.config.override(tma=0):
                 gen = run()
                 assert _lib.last_warp_variant() == "generic"
-            assert torch.equal(sweep, deal), (dsize, align, float((sweep - deal).abs().max()))
-            assert torch.equal(sweep, gen), (dsize, align, float((sweep - gen).abs().max()))
+            assert bits_equal(sweep, deal), (dsize, align, float((sweep - deal).abs().max()))
+            assert bits_equal(sweep, gen), (dsize, align, float((sweep - gen).abs().max()))
 
 
 def test_sweep_inside_a_cuda_graph():

@@ -15,17 +15,22 @@ DEV = "cuda"
 @pytest.mark.parametrize("border", ["reflect", "replicate", "constant"])
 @pytest.mark.parametrize("shape", [(2, 3, 64, 128), (1, 2, 70, 132), (3, 1, 34, 260), (1, 3, 4, 4), (1, 1, 1080, 1920)])
 def test_fused_pyrdown_equals_composition(border, shape):
-    """kb200_pyrdown_forward == filter2d (tiled 5x5) + F.interpolate(bilinear, align_corners=False), bit for bit."""
+    """kb200_pyrdown_forward == filter2d (tiled 5x5) + F.interpolate(bilinear, align_corners=False), bit for bit (-0 != +0), on
+    a random image and on one with NaN / Inf / -0 / subnormal texels at the tile seams.  Documented exception: no 3e38 texels --
+    the fused epilogue adds the four filtered taps before it scales them by 1/4, the composition scales each by 1/2 twice, so
+    four values near FLT_MAX overflow to Inf in the first and not in the second."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
     KT = K.geometry.transform
-    x = torch.rand(*shape, device=DEV)
-    K.config.set("fused_pyrdown", 0)
-    want = KT.pyrdown(x, border)
-    before = K._ops.launch_count
-    K.config.set("fused_pyrdown", 1)
-    got = KT.pyrdown(x, border)
-    assert K._ops.launch_count == before + 1, "the fused kernel did not run"
-    assert got.shape == want.shape and got.is_contiguous()
-    assert torch.equal(got, want), float((got - want).abs().max())
+    for x in (torch.rand(*shape, device=DEV), special_image(*shape, seed=1, huge=False)):
+        K.config.set("fused_pyrdown", 0)
+        want = KT.pyrdown(x, border)
+        before = K._ops.launch_count
+        K.config.set("fused_pyrdown", 1)
+        got = KT.pyrdown(x, border)
+        assert K._ops.launch_count == before + 1, "the fused kernel did not run"
+        assert got.shape == want.shape and got.is_contiguous()
+        assert bits_equal(got, want), float((got - want).abs().nan_to_num().max())
 
 
 def test_fused_pyrdown_golden_and_fallbacks():
@@ -55,13 +60,16 @@ def test_fused_pyrdown_golden_and_fallbacks():
 @pytest.mark.parametrize("mode,order", [("sobel", 1), ("diff", 1), ("sobel", 2), ("diff", 2)])
 @pytest.mark.parametrize("normalized", [True, False])
 def test_tiled_spatial_gradient_bit_identical(shape, mode, order, normalized):
-    """grad_tiled_kernel (KB200_TILED_GRADIENT=1) == spatial_gradient_fwd, bit for bit (same taps, same FMA order)."""
-    x = torch.rand(*shape, device=DEV)
-    K.config.set("tiled_gradient", 0)
-    want = K.filters.spatial_gradient(x, mode, order, normalized)
-    K.config.set("tiled_gradient", 1)
-    got = K.filters.spatial_gradient(x, mode, order, normalized)
-    assert got.shape == want.shape and torch.equal(got, want), float((got - want).abs().max())
+    """grad_tiled_kernel (KB200_TILED_GRADIENT=1) == spatial_gradient_fwd, bit for bit (same taps, same FMA order; -0 != +0), on a
+    random image and on one with NaN / Inf / -0 / subnormal texels at the tile seams."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
+    for x in (torch.rand(*shape, device=DEV), special_image(*shape, seed=2)):
+        K.config.set("tiled_gradient", 0)
+        want = K.filters.spatial_gradient(x, mode, order, normalized)
+        K.config.set("tiled_gradient", 1)
+        got = K.filters.spatial_gradient(x, mode, order, normalized)
+        assert got.shape == want.shape and bits_equal(got, want), float((got - want).abs().nan_to_num().max())
 
 
 @pytest.mark.parametrize("shape", [(2, 3, 64, 128), (1, 2, 70, 132), (1, 3, 1080, 1920)])
@@ -85,14 +93,17 @@ def test_tiled_sobel_bit_identical_and_golden(shape):
                                           if min(s[-2:]) > w // 2])  # a reflect fold needs an image larger than the half-window
 def test_band_walk_ssim_bit_identical(window, shape):
     """ssim_vwalk_kernel == the library's own differentiable composition (five one-pass blurs + torch elementwise ops, the path
-    taken when a gradient is needed), bit for bit."""
+    taken when a gradient is needed), bit for bit (-0 != +0); also with NaN / Inf / -0 / subnormal texels at the tile seams."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
     a = torch.rand(*shape, device=DEV)
     b = (a + 0.1 * torch.randn(*shape, device=DEV)).clamp(0, 1)
-    want = K.metrics.ssim(a.clone().requires_grad_(True), b, window).detach()
-    before = K._ops.launch_count
-    got = K.metrics.ssim(a, b, window)
-    assert K._ops.launch_count == before + 1, "the fused kernel did not run"
-    assert torch.equal(got, want), float((got - want).abs().max())
+    for a, b in ((a, b), (special_image(*shape, seed=3), b)):
+        want = K.metrics.ssim(a.clone().requires_grad_(True), b, window).detach()
+        before = K._ops.launch_count
+        got = K.metrics.ssim(a, b, window)
+        assert K._ops.launch_count == before + 1, "the fused kernel did not run"
+        assert bits_equal(got, want), float((got - want).abs().nan_to_num().max())
 
 
 def test_band_walk_ssim_many_segments_and_golden():
@@ -222,7 +233,10 @@ def test_tiled_backward_720p_and_goldens(stride1):
 @pytest.mark.parametrize("shape", [(2, 3, 64, 128), (1, 1, 70, 132), (3, 3, 270, 480), (1, 3, 1080, 1920)])
 def test_fused_undistort_equals_composition(ncoef, shape):
     """kb200_undistort_forward (lens model in registers) == distort_points (torch ops) + remap, bit for bit: the kernel
-    evaluates the reference's op sequence with one rounding per op on the exact integer grid."""
+    evaluates the reference's op sequence with one rounding per op on the exact integer grid.  The second image has NaN / Inf /
+    -0 / subnormal texels at the tile seams; the comparison is bit for bit with -0 != +0."""
+    from test_nonfinite_gpu import bits_equal, special_image
+
     KC = K.geometry.calibration
     B, C, H, W = shape
     g = torch.Generator().manual_seed(ncoef)
@@ -232,13 +246,14 @@ def test_fused_undistort_equals_composition(ncoef, shape):
     scale = torch.tensor([0.25, 0.08, 0.003, 0.003, 0.02, 0.05, 0.02, 0.004, 0.003, 0.001, 0.002, 0.0015, 0.0, 0.0])[:ncoef]
     dist = (torch.rand(B, ncoef, generator=g) - 0.5) * 2 * scale   # tilt terms zero: the fused envelope
     cam, dist = cam.to(DEV), dist.to(DEV)
-    K.config.set("fused_undistort", 0)
-    want = KC.undistort_image(img, cam, dist)
-    before = K._ops.launch_count
-    K.config.set("fused_undistort", 1)
-    got = KC.undistort_image(img, cam, dist)
-    assert K._ops.launch_count == before + 1, "the fused kernel did not run"
-    assert torch.equal(got, want), float((got - want).abs().max())
+    for img in (img, special_image(*shape, seed=ncoef)):
+        K.config.set("fused_undistort", 0)
+        want = KC.undistort_image(img, cam, dist)
+        before = K._ops.launch_count
+        K.config.set("fused_undistort", 1)
+        got = KC.undistort_image(img, cam, dist)
+        assert K._ops.launch_count == before + 1, "the fused kernel did not run"
+        assert bits_equal(got, want), float((got - want).abs().nan_to_num().max())
 
 
 def test_fused_undistort_golden_and_fallbacks():

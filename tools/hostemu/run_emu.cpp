@@ -58,10 +58,12 @@ static int fold(int q, int n, int border) {
   return q < 0 ? -q : 2 * (n - 1) - q;
 }
 static int failures = 0;
+// bit for bit, -0 != +0: every case of the fixed list and of the fuzz run holds to it (a kernel that seeded an accumulator
+// or folded a border differently from the scalar loop would show as a zero of the other sign)
 static void compare(const std::string& what, const float* got, const float* want, size_t n) {
   size_t bad = 0, first = 0;
   for (size_t i = 0; i < n; ++i)
-    if (memcmp(got + i, want + i, 4) != 0 && !(got[i] == 0.f && want[i] == 0.f)) {
+    if (memcmp(got + i, want + i, 4) != 0) {
       if (!bad) first = i;
       ++bad;
     }
@@ -71,6 +73,43 @@ static void compare(const std::string& what, const float* got, const float* want
   } else {
     printf("ok   %s\n", what.c_str());
   }
+}
+
+static int emu_strict_failures = 0;
+// bits equal (-0 != +0), or NaN on both sides: the device returns one canonical NaN, while on x86 the sign of a NaN produced
+// from two NaN operands depends on which operand the compiler put first in a commutative op
+static void compare_bits_or_nan(const std::string& what, const float* got, const float* want, size_t n) {
+  size_t bad = 0, first = 0;
+  for (size_t i = 0; i < n; ++i)
+    if (memcmp(got + i, want + i, 4) != 0 && !(got[i] != got[i] && want[i] != want[i])) {
+      if (!bad) first = i;
+      ++bad;
+    }
+  if (bad) {
+    printf("FAIL %-72s %zu / %zu differ in their bits, first at %zu: got %.9g want %.9g\n", what.c_str(), bad, n, first, got[first], want[first]);
+    ++failures;
+    ++emu_strict_failures;
+  } else {
+    printf("ok   %s\n", what.c_str());
+  }
+}
+
+// specials 1: NaN / +-Inf / -0 / subnormal / 1e-38 / 3e38 texels scattered; 2: the same, and the first plane all -0 (a
+// kernel that seeds an accumulator differently from the scalar loop shows there as +0 against -0).
+static void special_texels(float* x, size_t n, int specials, size_t plane = 0) {
+  if (!specials) return;
+  const float v[8] = {NAN, INFINITY, -INFINITY, -0.f, 1e-40f, -1e-41f, 1e-38f, 3e38f};
+  for (size_t i = 0; i < n; i += 97 + (rng() % 300)) x[i] = v[rng() % 8];
+  x[0] = 1e-40f;
+  x[n - 1] = -0.f;
+  if (specials >= 2 && plane && plane < n)
+    for (size_t i = 0; i < plane; ++i) x[i] = -0.f;
+}
+
+// the comparison of a case: with special texels bit for bit (-0 != +0, any NaN equals any NaN)
+static void compare_case(int specials, const std::string& what, const float* got, const float* want, size_t n) {
+  if (specials) compare_bits_or_nan(what + " specials=" + std::to_string(specials), got, want, n);
+  else compare(what, got, want, n);
 }
 
 // ------------------------------------------------------------------------------------------ separable filter
@@ -102,12 +141,13 @@ static void ref_sepfilter(const float* x, const float* kx, const float* ky, floa
 }
 
 template <int K, int BORDER>
-static void test_sepfilter(int B, int C, int H, int W, unsigned grid, bool lazy) {
+static void test_sepfilter(int B, int C, int H, int W, unsigned grid, bool lazy, int specials = 0) {
   emu::lazy_tma = lazy;
   const int planes = B * C;
   std::vector<float> xs, o1s, o2s;
   float* x = aligned(xs, (size_t)planes * H * W);
   for (size_t i = 0; i < (size_t)planes * H * W; ++i) x[i] = randv(1)[0];
+  special_texels(x, (size_t)planes * H * W, specials, (size_t)H * W);
   auto kx = randv((size_t)B * K, -1.f, 1.f), ky = randv(K, -1.f, 1.f);
   std::vector<float> want((size_t)planes * H * W);
   ref_sepfilter(x, kx.data(), ky.data(), want.data(), planes, C, H, W, B, K, BORDER);
@@ -119,7 +159,7 @@ static void test_sepfilter(int B, int C, int H, int W, unsigned grid, bool lazy)
     const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
     SepTiledParams p{kx.data(), ky.data(), o1, C, H, W, B, 1, planes, x, 0.f};
     emu::launch(grid, dim3(256), [&] { sepfilter_tiled_kernel<K, BORDER, false>(map, p); });
-    compare("sepfilter_tiled_kernel (verified on hw) " + tag, o1, want.data(), want.size());
+    compare_case(specials, "sepfilter_tiled_kernel (verified on hw) " + tag, o1, want.data(), want.size());
   }
   if (K <= 11) {  // unsharp_mask epilogue against the plain filter blended on the host (|w| < 0.5 and >= 0.5 take different forms)
     const float wts[2] = {0.3f, 2.0f};
@@ -129,7 +169,7 @@ static void test_sepfilter(int B, int C, int H, int W, unsigned grid, bool lazy)
     const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
     SepTiledParams p{kx.data(), ky.data(), o2, C, H, W, B, 1, planes, x, wt};
     emu::launch(grid, dim3(256), [&] { sepfilter_tiled_kernel<K, BORDER, true>(map, p); });
-    compare("sepfilter_tiled_kernel<LERP> vs lerp of the plain filter " + tag, o2, blended.data(), want.size());
+    compare_case(specials, "sepfilter_tiled_kernel<LERP> vs lerp of the plain filter " + tag, o2, blended.data(), want.size());
   }
 }
 
@@ -151,11 +191,12 @@ static void ref_filter2d(const float* x, const float* k, int nout, float* out, i
 }
 
 template <int BORDER>
-static void test_pyrdown(int planes, int H, int W, unsigned grid, bool lazy) {
+static void test_pyrdown(int planes, int H, int W, unsigned grid, bool lazy, int specials = 0) {
   emu::lazy_tma = lazy;
   std::vector<float> xs, os, fs;
   float* x = aligned(xs, (size_t)planes * H * W);
   for (size_t i = 0; i < (size_t)planes * H * W; ++i) x[i] = randv(1)[0];
+  special_texels(x, (size_t)planes * H * W, specials, (size_t)H * W);
   float taps[25];
   const float b5[5] = {1, 4, 6, 4, 1};
   for (int i = 0; i < 5; ++i)
@@ -175,22 +216,23 @@ static void test_pyrdown(int planes, int H, int W, unsigned grid, bool lazy) {
     float* o = aligned(fs, full.size());
     F2dTiledParams p{taps, o, 1, H, W, 1, planes};
     emu::launch(grid, dim3(256), [&] { filter2d_tiled_kernel<5, BORDER, false>(map, p); });
-    compare("filter2d_tiled_kernel<5> (verified on hw) " + tag, o, full.data(), full.size());
+    compare_case(specials, "filter2d_tiled_kernel<5> (verified on hw) " + tag, o, full.data(), full.size());
   }
   {
     float* o = aligned(os, want.size());
     F2dTiledParams p{taps, o, 1, H, W, 1, planes};
     emu::launch(grid, dim3(256), [&] { filter2d_tiled_kernel<5, BORDER, true>(map, p); });
-    compare("filter2d_tiled_kernel<5, DOWN2> (pyrdown)  " + tag, o, want.data(), want.size());
+    compare_case(specials, "filter2d_tiled_kernel<5, DOWN2> (pyrdown)  " + tag, o, want.data(), want.size());
   }
 }
 
 template <int K, int BORDER>
-static void test_filter2d(int planes, int H, int W, unsigned grid, bool lazy) {
+static void test_filter2d(int planes, int H, int W, unsigned grid, bool lazy, int specials = 0) {
   emu::lazy_tma = lazy;
   std::vector<float> xs, os;
   float* x = aligned(xs, (size_t)planes * H * W);
   for (size_t i = 0; i < (size_t)planes * H * W; ++i) x[i] = randv(1)[0];
+  special_texels(x, (size_t)planes * H * W, specials, (size_t)H * W);
   auto taps = randv(K * K, -1.f, 1.f);
   std::vector<float> want((size_t)planes * H * W);
   ref_filter2d(x, taps.data(), 1, want.data(), planes, H, W, K, BORDER);
@@ -198,13 +240,12 @@ static void test_filter2d(int planes, int H, int W, unsigned grid, bool lazy) {
   const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
   F2dTiledParams p{taps.data(), o, 1, H, W, 1, planes};
   emu::launch(grid, dim3(256), [&] { filter2d_tiled_kernel<K, BORDER, false>(map, p); });
-  compare("filter2d_tiled_kernel (verified on hw) K=" + std::to_string(K) + " border=" + std::to_string(BORDER) + " " + std::to_string(planes) + "x" +
+  compare_case(specials, "filter2d_tiled_kernel (verified on hw) K=" + std::to_string(K) + " border=" + std::to_string(BORDER) + " " + std::to_string(planes) + "x" +
               std::to_string(H) + "x" + std::to_string(W) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
           o, want.data(), want.size());
 }
 
 // ------------------------------------------------------------------------------------------ filter2d, zero-skipping (K 9..31)
-static int emu_strict_failures = 0;
 static void compare_bits(const std::string& what, const float* got, const float* want, size_t n) {  // -0 != +0 here
   size_t bad = 0, first = 0;
   for (size_t i = 0; i < n; ++i)
@@ -305,11 +346,12 @@ static void test_taps_all(bool lazy) {
 }
 
 template <int K, int NOUT, bool MAG>
-static void test_gradient(int planes, int H, int W, unsigned grid, bool lazy) {
+static void test_gradient(int planes, int H, int W, unsigned grid, bool lazy, int specials = 0) {
   emu::lazy_tma = lazy;
   std::vector<float> xs, os;
   float* x = aligned(xs, (size_t)planes * H * W);
   for (size_t i = 0; i < (size_t)planes * H * W; ++i) x[i] = randv(1)[0];
+  special_texels(x, (size_t)planes * H * W, specials, (size_t)H * W);
   GradTiledParams p;
   p.H = H; p.W = W; p.planes = planes; p.eps = 1e-6f;
   auto t = randv(NOUT * K * K, -1.f, 1.f);
@@ -329,14 +371,14 @@ static void test_gradient(int planes, int H, int W, unsigned grid, bool lazy) {
   p.out = aligned(os, want.size());
   const CUtensorMap map = emu::make_map(x, W, H, planes, SEPT_BW, SEPT_TH + K - 1, 1);
   emu::launch(grid, dim3(256), [&] { grad_tiled_kernel<K, NOUT, MAG ? GRAD_MAG : GRAD_PLANES>(map, p); });
-  compare("grad_tiled_kernel K=" + std::to_string(K) + " NOUT=" + std::to_string(NOUT) + (MAG ? " MAG " : "     ") + std::to_string(planes) + "x" +
+  compare_case(specials, "grad_tiled_kernel K=" + std::to_string(K) + " NOUT=" + std::to_string(NOUT) + (MAG ? " MAG " : "     ") + std::to_string(planes) + "x" +
               std::to_string(H) + "x" + std::to_string(W) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"),
           p.out, want.data(), want.size());
 }
 
 // ------------------------------------------------------------------------------------------ SSIM
 template <int K>
-static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy) {
+static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy, int specials = 0) {
   emu::lazy_tma = lazy;
   std::vector<float> as, bs, o1s, o2s;
   const size_t n = (size_t)planes * H * W;
@@ -346,6 +388,8 @@ static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy) {
     a[i] = randv(1)[0];
     b[i] = std::min(1.f, std::max(0.f, a[i] + randv(1, -0.1f, 0.1f)[0]));
   }
+  special_texels(a, n, specials, (size_t)H * W);
+  special_texels(b, n, specials ? 1 : 0);
   auto taps = randv(K, 0.f, 1.f);
   const float C1 = 1e-4f, C2 = 9e-4f, eps = 1e-12f;
   const std::string tag = "K=" + std::to_string(K) + " " + std::to_string(planes) + "x" + std::to_string(H) + "x" + std::to_string(W) +
@@ -364,27 +408,9 @@ static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy) {
     SsimVParams p{taps.data(), o2, planes, H, W, C1, C2, eps};
     emu::launch(grid, dim3(256), [&] { ssim_vwalk_kernel<K>(ma, mb, pa, pb, p); });
   }
-  compare("ssim_vwalk_kernel vs ssim_tiled_kernel " + tag, o2, o1, n);
+  compare_case(specials, "ssim_vwalk_kernel vs ssim_tiled_kernel " + tag, o2, o1, n);
 }
 
-
-// bits equal (-0 != +0), or NaN on both sides: the device returns one canonical NaN, while on x86 the sign of a NaN produced
-// from two NaN operands depends on which operand the compiler put first in a commutative op
-static void compare_bits_or_nan(const std::string& what, const float* got, const float* want, size_t n) {
-  size_t bad = 0, first = 0;
-  for (size_t i = 0; i < n; ++i)
-    if (memcmp(got + i, want + i, 4) != 0 && !(got[i] != got[i] && want[i] != want[i])) {
-      if (!bad) first = i;
-      ++bad;
-    }
-  if (bad) {
-    printf("FAIL %-72s %zu / %zu differ in their bits, first at %zu: got %.9g want %.9g\n", what.c_str(), bad, n, first, got[first], want[first]);
-    ++failures;
-    ++emu_strict_failures;
-  } else {
-    printf("ok   %s\n", what.c_str());
-  }
-}
 
 // ------------------------------------------------------------------------------------------ feature responses
 // Scalar restatement of kornia/feature/responses.py as this library composes it: spatial_gradient (replicate border,
@@ -394,14 +420,6 @@ static void compare_bits_or_nan(const std::string& what, const float* got, const
 static const float kSobel1[18] = {-1 / 8.f, 0, 1 / 8.f, -2 / 8.f, 0, 2 / 8.f, -1 / 8.f, 0, 1 / 8.f,
                                   -1 / 8.f, -2 / 8.f, -1 / 8.f, 0, 0, 0, 1 / 8.f, 2 / 8.f, 1 / 8.f};
 static const float kDiff1[18] = {0, 0, 0, -0.5f, 0, 0.5f, 0, 0, 0, 0, -0.5f, 0, 0, 0, 0, 0, 0.5f, 0};
-
-static void special_texels(float* x, size_t n, int specials) {
-  if (!specials) return;
-  const float v[8] = {NAN, INFINITY, -INFINITY, -0.f, 1e-40f, -1e-41f, 1e-38f, 3e38f};
-  for (size_t i = 0; i < n; i += 97 + (rng() % 300)) x[i] = v[rng() % 8];
-  x[0] = 1e-40f;
-  x[n - 1] = -0.f;
-}
 
 template <int KIND>
 static void test_corner(int planes, int C, int H, int W, bool diff, int specials, bool sigmas, unsigned grid, bool lazy) {
@@ -539,7 +557,7 @@ static float ref_remap_pixel(const float* plane, int H, int W, float mx, float m
   return a;
 }
 
-static void test_undistort(int B, int H, int W, bool lazy, bool strong = false) {
+static void test_undistort(int B, int H, int W, bool lazy, bool strong = false, int specials = 0) {
   emu::lazy_tma = lazy;
   emu::set_smem(remap_smem, sizeof(remap_smem));
   constexpr int C = 3;
@@ -547,6 +565,7 @@ static void test_undistort(int B, int H, int W, bool lazy, bool strong = false) 
   const size_t n = (size_t)B * C * H * W, npix = (size_t)B * H * W;
   float* src = aligned(ss, n);
   for (size_t i = 0; i < n; ++i) src[i] = randv(1)[0];
+  special_texels(src, n, specials, (size_t)H * W);
   std::vector<float> lens((size_t)B * 16);
   for (int b = 0; b < B; ++b) {
     // strong: a fish-eye-like model whose maps leave the 8-row windows (and partly the image): the exact per-pixel path
@@ -577,13 +596,13 @@ static void test_undistort(int B, int H, int W, bool lazy, bool strong = false) 
   {
     RemapTiledParams p{src, mx, my, o1, B, H, W, H, W, B, 0, nullptr};
     emu::launch3(grid, dim3(256), [&] { remap_tiled_kernel<3, KB200_ZEROS, true, false>(map, p); });
-    compare("remap_tiled_kernel (verified on hw) vs scalar bilinear " + tag, o1, want.data(), n);
+    compare_case(specials, "remap_tiled_kernel (verified on hw) vs scalar bilinear " + tag, o1, want.data(), n);
   }
   float* o2 = aligned(o2s, n);
   {
     RemapTiledParams p{src, nullptr, nullptr, o2, B, H, W, H, W, B, 0, lens.data()};
     emu::launch3(grid, dim3(256), [&] { remap_tiled_kernel<3, KB200_ZEROS, true, true>(map, p); });
-    compare("remap_tiled_kernel<LENS> (fused undistort) vs maps + remap " + tag, o2, o1, n);
+    compare_case(specials, "remap_tiled_kernel<LENS> (fused undistort) vs maps + remap " + tag, o2, o1, n);
   }
 }
 
@@ -598,7 +617,7 @@ static TmaBoxMaps box_maps(const float* src, int W, int H, int planes) {
 }
 
 template <bool PROJ, int PAD, int TW, int TH, int BW, int BH, int INTERP = KB200_BILINEAR, bool ALIGN = true>
-static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool lazy, bool tame) {
+static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool lazy, bool tame, int specials = 0) {
   emu::lazy_tma = lazy;
   emu::set_smem(tma_smem, sizeof(tma_smem));
   constexpr int C = 3;
@@ -606,6 +625,7 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
   std::vector<float> ss, o1s, o2s;
   float* src = aligned(ss, ns);
   for (size_t i = 0; i < ns; ++i) src[i] = randv(1)[0];
+  special_texels(src, ns, specials, (size_t)H * W);
   std::vector<float> m((size_t)B * 9), bx(w), by(h);
   for (int i = 0; i < w; ++i) bx[i] = ((float)i / (float)std::max(w - 1, 1) - 0.5f) * 2.f;
   for (int i = 0; i < h; ++i) by[i] = ((float)i / (float)std::max(h - 1, 1) - 0.5f) * 2.f;
@@ -615,6 +635,22 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
                         cosf(t) * (tame ? 0.995f : 0.97f), tame ? -0.008f : -0.03f, PROJ ? (tame ? 0.004f : 0.02f) : 0.f, PROJ ? (tame ? -0.003f : -0.015f) : 0.f, 1.f};
     memcpy(&m[(size_t)b * 9], M, sizeof(M));
   }
+  if (specials >= 2)  // degenerate normalised matrices in place of some samples
+    for (int b = 0; b < B; ++b) {
+      float* M = &m[(size_t)b * 9];
+      switch (rng() % 10) {
+        case 0: M[1] = NAN; break;                                          // a NaN entry
+        case 1: M[5] = INFINITY; break;                                     // an Inf entry
+        case 2: M[2] = 1e8f; break;                                         // pixel coordinates beyond the int range
+        case 3: M[2] = -1e30f; break;
+        case 4: for (int k = 0; k < 9; ++k) M[k] = 0.f; break;              // zero matrix: 0 / 0 under a projective map
+        case 5: M[0] = M[4] = 1e30f; break;                                 // a scale of 1e30
+        case 6: M[6] = PROJ ? 1.f : 0.f; M[7] = 0.f; M[8] = PROJ ? 0.f : 1.f; break;  // denominator exactly 0 on the middle column (odd w)
+        case 7: for (int k = 0; k < 9; ++k) M[k] *= 1e-20f; break;          // denominator ~1e-20, below the shared-reciprocal window
+        case 8: M[0] = -M[0]; M[4] = -M[4]; M[8] = -1.f; break;             // denominator negative everywhere
+        default: break;
+      }
+    }
   float* o1 = aligned(o1s, no);
   float* o2 = aligned(o2s, no);
   TmaWarpParams p{};
@@ -644,7 +680,7 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
       emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2, true>(map, q); });
       p.out = o3;  // keep the comparison below on o1
       p.out = o1;
-      compare("warp_fwd_tma<DYN> chunk=" + std::to_string(chunk) + " vs the static deal " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) +
+      compare_case(specials, "warp_fwd_tma<DYN> chunk=" + std::to_string(chunk) + " vs the static deal " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) +
                   " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager"), o3, o2, no);
     }
     // the sweep: every run drawn in raster order (static_pct 0), runs of 1, 2 and 3 tiles; then the same launch restricted to the
@@ -665,7 +701,7 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
       TmaWarpParams q = p;
       q.out = o3; q.counter = &counter; q.chunk_tiles = run; q.static_pct = 0;
       emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2, true>(map, q); });
-      compare("warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " vs its exact path" + tag, o3, o2, no);
+      compare_case(specials, "warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " vs its exact path" + tag, o3, o2, no);
       for (size_t i = 0; i < no; ++i) o3[i] = o4[i] = -5.f;
       counter = 0;
       q.only_class = CLASS_WIDE; q.m = m2.data();
@@ -673,10 +709,10 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
       TmaWarpParams r = p;
       r.out = o4; r.only_class = CLASS_WIDE; r.m = m2.data();
       emu::launch(grid, dim3(TMA_THREADS), [&] { warp_fwd_tma<C, INTERP, PAD, PROJ, ALIGN, TW, TH, BW, BH, 2>(map, r); });
-      compare("warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " wide class only vs the static deal" + tag, o3, o4, no);
+      compare_case(specials, "warp_fwd_tma<DYN> sweep run=" + std::to_string(run) + " wide class only vs the static deal" + tag, o3, o4, no);
     }
   }
-  compare(std::string("warp_fwd_tma (headline, verified on hw) vs its exact path ") + (PROJ ? "projective " : "affine ") + "interp=" + std::to_string(INTERP) + " pad=" + std::to_string(PAD) + " tile " +
+  compare_case(specials, std::string("warp_fwd_tma (headline, verified on hw) vs its exact path ") + (PROJ ? "projective " : "affine ") + "interp=" + std::to_string(INTERP) + " pad=" + std::to_string(PAD) + " tile " +
               std::to_string(TW) + "x" + std::to_string(TH) + " " + std::to_string(B) + "x3x" + std::to_string(H) + "x" + std::to_string(W) + " -> " + std::to_string(h) +
               "x" + std::to_string(w) + " grid=" + std::to_string(grid) + (lazy ? " lazy" : " eager") + (tame ? " tame" : " wild") + (ALIGN ? "" : " align_corners=False"),
           o1, o2, no);
@@ -684,7 +720,7 @@ static void test_forward(int B, int H, int W, int h, int w, unsigned grid, bool 
 
 // ------------------------------------------------------------------------------------------ tiled warp backward
 template <bool PROJ>
-static void test_backward(int B, int H, int W, int h, int w, unsigned grid, bool lazy, bool tame = false) {
+static void test_backward(int B, int H, int W, int h, int w, unsigned grid, bool lazy, bool tame = false, int specials = 0) {
   emu::lazy_tma = lazy;
   constexpr int C = 3;
   constexpr bool ALIGN = true;
@@ -694,6 +730,12 @@ static void test_backward(int B, int H, int W, int h, int w, unsigned grid, bool
   float* gout = aligned(gs, no);
   for (size_t i = 0; i < ns; ++i) src[i] = randv(1)[0];
   for (size_t i = 0; i < no; ++i) gout[i] = randv(1, -0.5f, 0.5f)[0];
+  // specials 1: special texels in the source, 2: in the upstream gradient.  Without 3e38: the fp64 reference does not overflow
+  // where fp32 sums of such terms do, so its classes would differ for a reason that is not the kernel's.
+  special_texels(specials == 2 ? gout : src, specials == 2 ? no : ns, specials ? 1 : 0);
+  for (float* v : {src, gout})
+    for (size_t i = 0, n = v == src ? ns : no; i < n; ++i)
+      if (v[i] == 3e38f) v[i] = -2.f;
   std::vector<float> m((size_t)B * 9), bx(w), by(h);
   for (int i = 0; i < w; ++i) bx[i] = ((float)i / (float)(w - 1) - 0.5f) * 2.f;
   for (int i = 0; i < h; ++i) by[i] = ((float)i / (float)(h - 1) - 0.5f) * 2.f;
@@ -797,7 +839,29 @@ static void test_backward(int B, int H, int W, int h, int w, unsigned grid, bool
     double mn = 0, md = 0;
     for (size_t i = 0; i < gm.size(); ++i) { mn += (gm[i] - gm_ref[i]) * (gm[i] - gm_ref[i]); md += gm_ref[i] * gm_ref[i]; }
     const double e_src = sqrt(num / den), e_m = sqrt(mn / md);
-    const bool ok = e_src < 2e-6 && worst < 2e-5 && e_m < 1e-4;
+    bool ok = e_src < 2e-6 && worst < 2e-5 && e_m < 1e-4;
+    if (specials) {  // the same non-finite classes entry by entry; the finite entries within the tolerances above
+      auto cls = [](double v) { return v != v ? 3 : v == INFINITY ? 1 : v == -INFINITY ? 2 : 0; };
+      size_t bad = 0;
+      num = den = worst = mn = md = 0;
+      for (size_t i = 0; i < ns; ++i) {
+        if (cls(g[i]) != cls(gsrc_ref[i])) { ++bad; continue; }
+        if (cls(g[i])) continue;
+        const double d = (double)g[i] - gsrc_ref[i];
+        num += d * d; den += gsrc_ref[i] * gsrc_ref[i];
+        worst = std::max(worst, fabs(d));
+      }
+      for (size_t i = 0; i < gm.size(); ++i) {
+        if (cls(gm[i]) != cls(gm_ref[i])) { ++bad; continue; }
+        if (!cls(gm[i])) { mn += (gm[i] - gm_ref[i]) * (gm[i] - gm_ref[i]); md += gm_ref[i] * gm_ref[i]; }
+      }
+      const double es = den > 0 ? sqrt(num / den) : 0.0, em = md > 0 ? sqrt(mn / md) : 0.0;
+      ok = bad == 0 && es < 2e-6 && worst < 2e-5 && em < 1e-4;
+      printf("%s %-58s %s  specials=%d: %zu class mismatches, finite d/dsrc rel-L2 %.2e max-abs %.2e, d/dM rel-L2 %.2e\n", ok ? "ok  " : "FAIL", name,
+             tag.c_str(), specials, bad, es, worst, em);
+      if (!ok) ++failures;
+      return;
+    }
     printf("%s %-58s %s  d/dsrc rel-L2 %.2e max-abs %.2e, d/dM rel-L2 %.2e\n", ok ? "ok  " : "FAIL", name, tag.c_str(), e_src, worst, e_m);
     if (!ok) ++failures;
   };
@@ -1038,13 +1102,67 @@ static void probe_forward() {
          emu_careful_pixels, H * W);
 }
 
+// The special-value list (also alone: run_emu --specials): NaN / +-Inf / -0 / subnormal / 1e-38 / 3e38 texels and a plane of
+// -0 through every tiled kernel, compared bit for bit (-0 != +0); the headline forward kernel (both tile shapes, every
+// interpolation) also under degenerate matrices; the tiled backward with special texels and special upstream gradients.
+static void test_specials_all(bool lazy) {
+  for (int sp = 1; sp <= 2; ++sp) {
+    test_sepfilter<11, KB200_REFLECT>(2, 3, 70, 132, 5, lazy, sp);
+    test_sepfilter<3, KB200_CONSTANT>(1, 2, 33, 68, 2, lazy, sp);
+    test_sepfilter<17, KB200_REPLICATE>(1, 2, 97, 140, 3, lazy, sp);
+    test_filter2d<3, KB200_REFLECT>(3, 70, 132, 4, lazy, sp);
+    test_filter2d<5, KB200_CONSTANT>(2, 33, 68, 2, lazy, sp);
+    test_filter2d<7, KB200_REPLICATE>(2, 40, 72, 3, lazy, sp);
+    test_pyrdown<KB200_REFLECT>(3, 70, 132, 4, lazy, sp);
+    test_pyrdown<KB200_CONSTANT>(2, 34, 68, 3, lazy, sp);
+    test_gradient<3, 2, false>(3, 70, 132, 4, lazy, sp);
+    test_gradient<3, 2, true>(2, 33, 260, 3, lazy, sp);
+    test_gradient<5, 3, false>(2, 97, 136, 5, lazy, sp);
+    test_ssim<11>(3, 70, 132, 4, lazy, sp);
+    test_ssim<7>(2, 33, 68, 3, lazy, sp);
+    test_undistort(2, 70, 132, lazy, false, sp);
+    test_undistort(2, 97, 200, lazy, true, sp);
+    test_forward<true, KB200_ZEROS, 64, 32, 72, 40>(3, 70, 132, 50, 101, 2, lazy, false, sp);
+    test_forward<true, KB200_ZEROS, 64, 32, 72, 40>(4, 96, 200, 96, 199, 3, lazy, true, sp);
+    test_forward<false, KB200_BORDER, 64, 32, 72, 40>(3, 64, 128, 70, 133, 4, lazy, true, sp);
+    test_forward<true, KB200_REFLECTION, 64, 32, 72, 40>(3, 70, 132, 70, 131, 3, lazy, false, sp);
+    test_forward<true, KB200_FILL, 64, 32, 72, 40>(3, 70, 132, 64, 121, 2, lazy, true, sp);
+    test_forward<true, KB200_ZEROS, 32, 32, 56, 56>(3, 70, 132, 70, 131, 3, lazy, false, sp);
+    test_forward<true, KB200_REFLECTION, 32, 32, 56, 56>(3, 70, 132, 70, 131, 2, lazy, true, sp);
+    test_forward<true, KB200_ZEROS, 64, 32, 72, 40, KB200_NEAREST>(3, 70, 132, 70, 131, 3, lazy, true, sp);
+    test_forward<true, KB200_BORDER, 64, 32, 72, 40, KB200_BICUBIC>(3, 70, 132, 70, 131, 2, lazy, true, sp);
+    test_forward<false, KB200_REFLECTION, 64, 32, 72, 40, KB200_BICUBIC>(3, 64, 128, 70, 133, 3, lazy, false, sp);
+    test_backward<true>(3, 70, 132, 70, 132, 2, lazy, false, sp);
+    test_backward<false>(3, 64, 128, 50, 96, 3, lazy, true, sp);
+  }
+}
+
 static void fuzz(int rounds) {
   std::mt19937 g(20260923);
   auto pick = [&](int lo, int hi) { return lo + (int)(g() % (unsigned)(hi - lo + 1)); };
   for (int r = 0; r < rounds; ++r) {
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
-    switch (pick(0, 46)) {
+    switch (pick(0, 50)) {
+      case 47:
+      case 48: {  // special texels (and degenerate matrices) through the tiled filters and the headline forward kernel
+        const int sp = pick(1, 2);
+        const int which = pick(0, 5);
+        if (which == 0 && H > 5 && W > 5) test_sepfilter<11, KB200_REFLECT>(1, planes, H, W, grid, lazy, sp);
+        else if (which == 1) test_filter2d<5, KB200_CONSTANT>(planes, H, W, grid, lazy, sp);
+        else if (which == 2 && H > 2) test_gradient<5, 3, false>(planes, H, W, grid, lazy, sp);
+        else if (which == 3 && H > 1) test_forward<true, KB200_ZEROS, 64, 32, 72, 40>(3, H, W, std::max(1, H - pick(0, 5)), std::max(4, W - pick(0, 3)), grid, lazy, pick(0, 1), sp);
+        else if (which == 4 && H > 1) test_forward<true, KB200_REFLECTION, 32, 32, 56, 56, KB200_BICUBIC>(3, H, W, H, std::max(4, W - 1), grid, lazy, pick(0, 1), sp);
+        else if (H > 3 && W > 3) test_ssim<7>(planes, H, W, grid, lazy, sp);
+        break;
+      }
+      case 49:
+      case 50: {  // remap / fused undistort and the tiled backward with special values
+        const int sp = pick(1, 2);
+        if (pick(0, 1) && H > 1) test_undistort(pick(1, 2), H, W, lazy, pick(0, 1), sp);
+        else if (H > 1 && W > 4) test_backward<true>(3, H, W, std::max(2, H - pick(0, 3)), std::max(8, W - 4 * pick(0, 2)), grid, lazy, pick(0, 1), sp);
+        break;
+      }
       case 44:
       case 45:
       case 46: {  // feature responses: Harris / GFTT / Hessian, both stencil modes, C 1..3, sigmas, special texels
@@ -1129,6 +1247,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--responses") {
     for (int lazy = 0; lazy < 2; ++lazy) test_responses_all(lazy);
     printf("%s: %d failing comparisons (feature responses, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--specials") {
+    for (int lazy = 0; lazy < 2; ++lazy) test_specials_all(lazy);
+    printf("%s: %d failing comparisons (special values, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 3 && std::string(argv[1]) == "--fuzz") {
