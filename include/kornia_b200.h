@@ -249,6 +249,23 @@ int kb200_feature_response_forward(const void* x, const double* stencil, const v
                                    int kind, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * One octave of ScalePyramid (geometry/transform/pyramid.py:367-384: a reflect-bordered separable Gaussian per level,
+ * each of the level before it, then torch.stack) in ONE kernel: 4 B read + 4 B written per element and level.
+ *   x       (planes,H,W) device, the octave's seed (the input, its 2x upsample, or the bilinear octave seed)
+ *   taps    HOST pointer to the taps of ksizes[0], ksizes[1], ... in that order, doubles exact in fp32
+ *   ksizes  HOST pointer to L tap counts: ksizes[0] the initial blur of level 0 (0: level 0 is x itself), ksizes[l] the
+ *           blur from level l-1 to level l
+ *   out     (planes,L,H,W): every level of the octave
+ * Each level is a row pass, then a column pass, with ascending taps, one FMA per tap from 0 and the reflect border of
+ * the level it filters: bit-identical to L - 1 (or L) calls of kb200_sepfilter_forward.  fp32 with W % 4 == 0,
+ * 16-byte aligned buffers, every tap count <= min(H, W), and one of the chains 13 | 11 13 17 21 25, 13 | 11 13 17 21,
+ * 11 | 11 13 17 21 25, 0 | 11 13 17 21 25, 0 | 11 13 17 21 only: anything else returns KB200_EUNSUPPORTED and the
+ * host composes the octave.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_scale_octave_forward(const void* x, const double* taps, const int* ksizes, int L, void* out, int planes, int H, int W,
+                               int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

@@ -22,8 +22,10 @@ def install(kornia_module=None) -> None:
     """Rebind the hot-path functions (and the four callers that have a fused kernel of their own here:
     ``get_perspective_transform``, ``spatial_gradient``, ``sobel``, ``ssim``, plus ``motion_blur`` and
     ``get_motion_kernel2d``, whose kernel must be built on the GPU, and the ``harris_response`` / ``gftt_response`` /
-    ``hessian_response`` of the classical detectors) on an imported ``kornia`` package.  A defining
-    module the package lacks is skipped.
+    ``hessian_response`` of the classical detectors, and the ``ScalePyramid`` class their scale-space detectors build) on an
+    imported ``kornia`` package.  A defining module the package lacks, or a name its module does not define, is skipped.
+    Rebinding ``ScalePyramid`` affects modules constructed afterwards: a ``ScaleSpaceDetector`` built before ``install()``
+    keeps the reference pyramid it holds.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -57,6 +59,8 @@ def install(kornia_module=None) -> None:
         "harris_response": ("feature.responses", feature.harris_response),
         "gftt_response": ("feature.responses", feature.gftt_response),
         "hessian_response": ("feature.responses", feature.hessian_response),
+        # a class: ScaleSpaceDetector (feature/scale_space_detector.py) and integrated.py build theirs from this name
+        "ScalePyramid": ("geometry.transform.pyramid", geometry.transform.ScalePyramid),
     }
     originals = {}
     for name, (mod, fn) in defining.items():
@@ -66,6 +70,8 @@ def install(kornia_module=None) -> None:
             if e.name is not None and (prefix + mod).startswith(e.name):
                 continue
             raise
+        if (m, name) not in _PATCHED and not hasattr(m, name):  # a package whose module does not define it: nothing to rebind
+            continue
         originals[name] = (_PATCHED.get((m, name), getattr(m, name)), fn)
     for modname, m in list(sys.modules.items()):
         if m is None or not (modname == k.__name__ or modname.startswith(prefix)):

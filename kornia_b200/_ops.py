@@ -768,6 +768,24 @@ _define("feature_response_fwd",
                                                                       torch.empty_like(x, memory_format=torch.contiguous_format))[1])
 
 
+def _scale_octave_cuda(x, taps, ksizes):
+    _require_cuda(x, "input")
+    xc = x.contiguous()
+    B, C, H, W = xc.shape
+    L = len(ksizes)
+    out = torch.empty((B, C, L, H, W), device=x.device, dtype=x.dtype)
+    host_taps = (ctypes.c_double * max(len(taps), 1))(*taps)
+    host_k = (ctypes.c_int * L)(*ksizes)
+    with torch.cuda.device(x.device), _Timed("scale_octave_forward", x):
+        _lib.call("kb200_scale_octave_forward", _ptr(xc), host_taps, host_k, L, _ptr(out), B * C, H, W, _dtype_code(x), _stream(x))
+    _bump()
+    return out
+
+
+_define("scale_octave_fwd", "(Tensor x, float[] taps, int[] ksizes) -> Tensor", _scale_octave_cuda,
+        lambda x, taps, ksizes: x.new_empty((x.shape[0], x.shape[1], len(ksizes), x.shape[2], x.shape[3])))
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -945,4 +963,5 @@ OPERATORS: Tuple[str, ...] = (
     "warp_fwd", "warp_bwd", "warp_prelude", "warp_prelude_bwd", "remap_fwd", "remap_bwd", "filter2d_fwd", "filter2d_bwd_input",
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
+    "scale_octave_fwd",
 )

@@ -15,6 +15,7 @@
 #include "gradient.cuh"
 #include "ssim_vwalk.cuh"
 #include "corner_vwalk.cuh"
+#include "octave_vwalk.cuh"
 #include "gradient_tiled.cuh"
 
 namespace kb200 {
@@ -609,6 +610,20 @@ int kb200_feature_response_forward(const void* x, const double* stencil, const v
   if (rc == KB200_EUNSUPPORTED)
     set_error("the fused response kernels need rows that are a multiple of 4 floats (16-byte aligned) and an image larger than the stencil, "
               "got H=%d W=%d", H, W);
+  return rc;
+}
+
+int kb200_scale_octave_forward(const void* x, const double* taps, const int* ksizes, int L, void* out, int planes, int H, int W, int dtype,
+                               void* stream) {
+  KB_CHECK_ARG(x && taps && ksizes && out, "null pointer argument");
+  KB_CHECK_ARG(planes > 0 && H > 0 && W > 0 && L > 0, "bad sizes planes=%d L=%d H=%d W=%d", planes, L, H, W);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  for (int l = 0; l < L; ++l) KB_CHECK_ARG(ksizes[l] >= (l == 0 ? 0 : 1), "bad tap count %d of level %d", ksizes[l], l);
+  const int rc = dtype == KB200_F32 ? octave_vwalk_forward((const float*)x, taps, ksizes, L, (float*)out, planes, H, W, (cudaStream_t)stream)
+                                    : KB200_EUNSUPPORTED;
+  if (rc == KB200_EUNSUPPORTED)
+    set_error("the fused octave kernel is fp32 only, for the instantiated tap chains, with every tap count <= min(H, W) and rows that are a "
+              "multiple of 4 floats (16-byte aligned), got L=%d H=%d W=%d", L, H, W);
   return rc;
 }
 

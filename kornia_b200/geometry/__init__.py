@@ -12,6 +12,7 @@ from .transform import (
     get_rotation_matrix2d,
     pyrdown,
     pyrup,
+    ScalePyramid,
     remap,
     rescale,
     resize,
@@ -24,6 +25,6 @@ from .transform import (
 )
 
 __all__ = ["transform", "calibration", "undistort_image", "distort_points", "pyrdown", "pyrup", "build_pyramid",
-           "build_laplacian_pyramid", "resize", "rescale", "remap", "warp_affine", "warp_perspective", "affine", "rotate", "translate", "scale", "shear",
+           "build_laplacian_pyramid", "ScalePyramid", "resize", "rescale", "remap", "warp_affine", "warp_perspective", "affine", "rotate", "translate", "scale", "shear",
            "crop_and_resize", "center_crop", "crop_by_boxes", "crop_by_transform_mat", "get_perspective_transform",
            "get_rotation_matrix2d"]

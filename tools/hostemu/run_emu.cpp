@@ -15,6 +15,7 @@
 #include "../../kornia_b200/csrc/gradient_tiled.cuh"
 #include "../../kornia_b200/csrc/ssim_vwalk.cuh"
 #include "../../kornia_b200/csrc/corner_vwalk.cuh"
+#include "../../kornia_b200/csrc/octave_vwalk.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -30,6 +31,7 @@ alignas(128) unsigned char f2dt_smem[128 * 1024];
 alignas(128) unsigned char gradt_smem[256 * 1024];
 alignas(128) unsigned char ssimv_smem[256 * 1024];
 alignas(128) unsigned char corner_smem[256 * 1024];
+alignas(128) unsigned char oct_smem[256 * 1024];
 alignas(128) float ssim_smem[64 * 1024];
 alignas(128) unsigned char remap_smem[256 * 1024];
 alignas(128) unsigned char tma_smem[256 * 1024];
@@ -411,6 +413,97 @@ static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy, int sp
   compare_case(specials, "ssim_vwalk_kernel vs ssim_tiled_kernel " + tag, o2, o1, n);
 }
 
+
+// ------------------------------------------------------------------------------------------ ScalePyramid octave
+// Scalar restatement of one octave as this library composes it: level 0 the source or its filter2d_separable with the
+// initial taps, level l the filter2d_separable of level l-1 (row pass, then column pass, ascending FMA from 0, reflect
+// border of the level it filters).  Compared bit for bit (-0 != +0, NaN equals NaN) with octave_vwalk_kernel, whose
+// output is prefilled with a value no level produces.
+template <typename CH>
+static void test_octave(int planes, int H, int W, int specials, unsigned grid) {
+  constexpr int L = CH::L;
+  const size_t HW = (size_t)H * W, n = (size_t)planes * HW;
+  std::vector<float> xs, os;
+  float* x = aligned(xs, n);
+  for (size_t i = 0; i < n; ++i) x[i] = randv(1, -1.f, 2.f)[0];
+  special_texels(x, n, specials, HW);
+  OctaveParams p{};
+  for (int l = 0; l < L; ++l) {
+    const int K = CH::K[l];
+    float s = 0.f;
+    const float sig = 0.15f * K + 0.1f * (float)l;
+    for (int j = 0; j < K; ++j) s += (p.taps[l][j] = expf(-0.5f * (float)((j - K / 2) * (j - K / 2)) / (sig * sig)));
+    for (int j = 0; j < K; ++j) p.taps[l][j] /= s;
+  }
+  std::vector<float> want(n * L), row(HW);
+  for (int pl = 0; pl < planes; ++pl) {
+    for (int l = 0; l < L; ++l) {
+      float* dst = want.data() + ((size_t)pl * L + l) * HW;
+      const float* prev = l == 0 ? x + pl * HW : dst - HW;
+      if (l == 0 && !CH::BLUR0) {
+        std::copy(prev, prev + HW, dst);
+        continue;
+      }
+      const int K = CH::K[l], h = K / 2;
+      for (int y = 0; y < H; ++y)
+        for (int xx = 0; xx < W; ++xx) {
+          float a = 0.f;
+          for (int j = 0; j < K; ++j) a = fmaf(p.taps[l][j], prev[(size_t)y * W + fold(xx + j - h, W, KB200_REFLECT)], a);
+          row[y * W + xx] = a;
+        }
+      for (int y = 0; y < H; ++y)
+        for (int xx = 0; xx < W; ++xx) {
+          float a = 0.f;
+          for (int i = 0; i < K; ++i) a = fmaf(p.taps[l][i], row[(size_t)fold(y + i - h, H, KB200_REFLECT) * W + xx], a);
+          dst[(size_t)y * W + xx] = a;
+        }
+    }
+  }
+  float* out = aligned(os, n * L);
+  std::fill(out, out + n * L, -777.f);
+  p.src = x;
+  p.out = out;
+  p.planes = planes;
+  p.H = H;
+  p.W = W;
+  emu::launch(grid, dim3(OCT_NT), [&] { octave_vwalk_kernel<CH>(p); });
+  std::string chain = std::to_string(CH::K[0] * CH::BLUR0);
+  for (int l = 1; l < L; ++l) chain += "," + std::to_string(CH::K[l]);
+  compare_bits_or_nan("octave_vwalk_kernel [" + chain + "] " + std::to_string(planes) + "x" + std::to_string(H) + "x" + std::to_string(W) +
+                          (specials ? " special texels" : "") + " grid=" + std::to_string(grid),
+                      out, want.data(), n * L);
+}
+
+using OctDefault = OctaveChain<13, 11, 13, 17, 21, 25>;
+using OctDetector = OctaveChain<13, 11, 13, 17, 21>;
+using OctDouble = OctaveChain<11, 11, 13, 17, 21, 25>;
+using OctCopy6 = OctaveChain<0, 11, 13, 17, 21, 25>;
+using OctCopy5 = OctaveChain<0, 11, 13, 17, 21>;
+
+// One octave of a chain on a shape and grid, with finite and special texels.
+template <typename CH>
+static void test_octave_both(int planes, int H, int W, unsigned grid) {
+  test_octave<CH>(planes, H, W, 0, grid);
+  test_octave<CH>(planes, H, W, 2, grid);
+}
+
+// The fixed list (also alone: run_emu --octave): every instantiation in both stage-0 modes; the smallest side equal to the
+// largest tap count (25 x 28, 21 x 60 for the 21-tap chains); widths 28, 60, 132 (a band of 4 columns); heights that are
+// not a multiple of the 16-row step; grids larger than the number of bands (segments that start in the middle of a band,
+// after the priming steps) and grids that do not divide them.
+static void test_octave_all() {
+  test_octave_both<OctDefault>(2, 25, 28, 1);
+  test_octave_both<OctDefault>(1, 70, 132, 3);
+  test_octave_both<OctDefault>(2, 97, 60, 7);
+  test_octave_both<OctDetector>(1, 21, 60, 2);
+  test_octave_both<OctDetector>(2, 61, 132, 5);
+  test_octave_both<OctDouble>(1, 33, 260, 4);
+  test_octave_both<OctDouble>(3, 26, 28, 2);
+  test_octave_both<OctCopy6>(1, 25, 132, 2);
+  test_octave_both<OctCopy6>(2, 83, 60, 9);
+  test_octave_both<OctCopy5>(1, 21, 28, 1);
+  test_octave_both<OctCopy5>(2, 140, 68, 11);
+}
 
 // ------------------------------------------------------------------------------------------ feature responses
 // Scalar restatement of kornia/feature/responses.py as this library composes it: spatial_gradient (replicate border,
@@ -1140,7 +1233,20 @@ static void test_specials_all(bool lazy) {
 static void fuzz(int rounds) {
   std::mt19937 g(20260923);
   auto pick = [&](int lo, int hi) { return lo + (int)(g() % (unsigned)(hi - lo + 1)); };
+  std::mt19937 go(20261017);  // the octave cases draw from their own stream, so the other cases stay what they were
+  auto opick = [&](int lo, int hi) { return lo + (int)(go() % (unsigned)(hi - lo + 1)); };
   for (int r = 0; r < rounds; ++r) {
+    if (r % 10 == 9) {  // ScalePyramid octave: any chain, both stage-0 modes, sides from the largest tap count up, any grid
+      const int which = opick(0, 4), planes = opick(1, 2), sp = opick(0, 2);
+      const unsigned grid = (unsigned)opick(1, 12);
+      const int kmax = which == 1 || which == 4 ? 21 : 25;
+      const int H = opick(kmax, 120), W = 4 * opick((kmax + 3) / 4, 70);
+      if (which == 0) test_octave<OctDefault>(planes, H, W, sp, grid);
+      else if (which == 1) test_octave<OctDetector>(planes, H, W, sp, grid);
+      else if (which == 2) test_octave<OctDouble>(planes, H, W, sp, grid);
+      else if (which == 3) test_octave<OctCopy6>(planes, H, W, sp, grid);
+      else test_octave<OctCopy5>(planes, H, W, sp, grid);
+    }
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
     switch (pick(0, 50)) {
@@ -1247,6 +1353,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--responses") {
     for (int lazy = 0; lazy < 2; ++lazy) test_responses_all(lazy);
     printf("%s: %d failing comparisons (feature responses, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--octave") {
+    test_octave_all();
+    printf("%s: %d failing comparisons (ScalePyramid octave, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {

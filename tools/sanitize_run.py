@@ -81,5 +81,7 @@ for shape in ((3, 100, 192, 3), (2, 70, 132, 1), (1, 33, 45, 3)):  # the last on
     frames = torch.randint(0, 256, shape, generator=g, dtype=torch.uint8).to(dev)
     camq = torch.tensor([[0.8 * shape[2], 0.0, shape[2] / 2], [0.0, 0.8 * shape[2], shape[1] / 2], [0.0, 0.0, 1.0]], device=dev).expand(shape[0], 3, 3).contiguous()
     KC.undistort_image_from_uint8(frames, camq, torch.tensor([[-0.2, 0.05, 0.001, -0.002, 0.01]], device=dev).expand(shape[0], 5).contiguous())
+# ScalePyramid: the octave kernel (blur and copy stages, a band of 4 columns, more CTAs than bands), tiny octaves composed
+KT.ScalePyramid(min_size=8)(torch.rand(2, 1, 100, 132, generator=g).to(dev))
 torch.cuda.synchronize()
 print("sanitize workload done")
