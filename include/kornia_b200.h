@@ -266,6 +266,24 @@ int kb200_scale_octave_forward(const void* x, const double* taps, const int* ksi
                                int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Non-maximum suppression (geometry/subpix/nms.py) in ONE kernel per call: 4 B read and 1 B (mask) or 4 B (values)
+ * written per element, instead of one ATen kernel per neighbour comparison.
+ *   x     fp32 source whose H x W planes are dense; sB, sC (and sL) are the element strides of b, c (and the level), so a
+ *         permuted (B, C, L, H, W) view is read in place
+ *   out   contiguous (B, C, H, W) / (B, C, L, H, W): uint8 0/1 masks, or fp32 x * mask (values = 1, mode = 1)
+ * kb200_nms2d_forward: NonMaximaSuppression2d((k, k)) for odd k = 3..31; k = 3, 5, 7 compare with the k*k - 1 neighbours
+ * and leave the (k - 1) / 2 border False, k >= 9 follows the reference's one-hot F.conv2d of the replicate-padded
+ * image (0 joins the neighbour set; a window holding a non-finite texel is False).  Anything else returns
+ * KB200_EUNSUPPORTED and the host composes the reference's op sequence.
+ * kb200_nms3d_forward: NonMaximaSuppression3d((3, 3, 3)); mode 0 the maxima mask, 1 the maxima values, 2 nms3d_minmax's
+ * maxima (out0) and minima (out1) masks.  Border levels, rows and columns are False.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_nms2d_forward(const void* x, void* out, int B, int C, int H, int W, long long sB, long long sC, int k, int values, int dtype,
+                        void* stream);
+int kb200_nms3d_forward(const void* x, void* out0, void* out1, int B, int C, int L, int H, int W, long long sB, long long sC,
+                        long long sL, int mode, int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

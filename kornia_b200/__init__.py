@@ -22,10 +22,12 @@ def install(kornia_module=None) -> None:
     """Rebind the hot-path functions (and the four callers that have a fused kernel of their own here:
     ``get_perspective_transform``, ``spatial_gradient``, ``sobel``, ``ssim``, plus ``motion_blur`` and
     ``get_motion_kernel2d``, whose kernel must be built on the GPU, and the ``harris_response`` / ``gftt_response`` /
-    ``hessian_response`` of the classical detectors, and the ``ScalePyramid`` class their scale-space detectors build) on an
-    imported ``kornia`` package.  A defining module the package lacks, or a name its module does not define, is skipped.
-    Rebinding ``ScalePyramid`` affects modules constructed afterwards: a ``ScaleSpaceDetector`` built before ``install()``
-    keeps the reference pyramid it holds.
+    ``hessian_response`` of the classical detectors, the ``ScalePyramid`` class their scale-space detectors build, and the
+    non-maximum suppression ``nms2d`` / ``nms3d`` / ``nms3d_minmax`` / ``NonMaximaSuppression2d`` /
+    ``NonMaximaSuppression3d`` of the detectors and the sub-pixel refiners) on an imported ``kornia`` package.  A defining
+    module the package lacks, or a name its module does not define, is skipped.  Rebinding a class affects modules
+    constructed afterwards: a ``ScaleSpaceDetector`` or ``MultiResolutionDetector`` built before ``install()`` keeps the
+    reference pyramid and the reference ``NonMaximaSuppression2d`` it holds.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -61,6 +63,12 @@ def install(kornia_module=None) -> None:
         "hessian_response": ("feature.responses", feature.hessian_response),
         # a class: ScaleSpaceDetector (feature/scale_space_detector.py) and integrated.py build theirs from this name
         "ScalePyramid": ("geometry.transform.pyramid", geometry.transform.ScalePyramid),
+        # ScaleSpaceDetector, MultiResolutionDetector, DISK, XFeat, ALIKED and the subpix refiners import these by name
+        "nms2d": ("geometry.subpix.nms", geometry.subpix.nms2d),
+        "nms3d": ("geometry.subpix.nms", geometry.subpix.nms3d),
+        "nms3d_minmax": ("geometry.subpix.nms", geometry.subpix.nms3d_minmax),
+        "NonMaximaSuppression2d": ("geometry.subpix.nms", geometry.subpix.NonMaximaSuppression2d),
+        "NonMaximaSuppression3d": ("geometry.subpix.nms", geometry.subpix.NonMaximaSuppression3d),
     }
     originals = {}
     for name, (mod, fn) in defining.items():

@@ -786,6 +786,65 @@ _define("scale_octave_fwd", "(Tensor x, float[] taps, int[] ksizes) -> Tensor", 
         lambda x, taps, ksizes: x.new_empty((x.shape[0], x.shape[1], len(ksizes), x.shape[2], x.shape[3])))
 
 
+def _dense_planes(x: torch.Tensor) -> torch.Tensor:
+    """``x`` itself when each H x W plane is dense (the kernels take the outer strides), else a contiguous copy."""
+    H, W = x.shape[-2:]
+    if (W == 1 or x.stride(-1) == 1) and (H == 1 or x.stride(-2) == W):
+        return x
+    return x.contiguous()
+
+
+def _nms2d_cuda(x, k, mask_only):
+    _require_cuda(x, "input")
+    B, C, H, W = x.shape
+    out = torch.empty((B, C, H, W), device=x.device, dtype=torch.bool if mask_only else x.dtype)
+    if out.numel() == 0:
+        return out
+    xs = _dense_planes(x)
+    with torch.cuda.device(x.device), _Timed("nms2d_forward", x):
+        _lib.call("kb200_nms2d_forward", _ptr(xs), _ptr(out), B, C, H, W, xs.stride(0), xs.stride(1), k, 0 if mask_only else 1,
+                  _dtype_code(x), _stream(x))
+    _bump()
+    return out
+
+
+_define("nms2d_fwd", "(Tensor x, int k, bool mask_only) -> Tensor", _nms2d_cuda,
+        lambda x, k, mask_only: x.new_empty(x.shape, dtype=torch.bool if mask_only else x.dtype))
+
+NMS3_MAX_MASK, NMS3_MAX_VALUES, NMS3_MINMAX = 0, 1, 2  # mode of kb200_nms3d_forward
+
+
+def _nms3d_call(x, out0, out1, mode):
+    _require_cuda(x, "input")
+    if out0.numel() == 0:
+        return
+    B, C, L, H, W = x.shape
+    xs = _dense_planes(x)
+    with torch.cuda.device(x.device), _Timed("nms3d_forward", x):
+        _lib.call("kb200_nms3d_forward", _ptr(xs), _ptr(out0), _ptr(out1), B, C, L, H, W, xs.stride(0), xs.stride(1), xs.stride(2), mode,
+                  _dtype_code(x), _stream(x))
+    _bump()
+
+
+def _nms3d_cuda(x, mask_only):
+    out = torch.empty(x.shape, device=x.device, dtype=torch.bool if mask_only else x.dtype)
+    _nms3d_call(x, out, None, NMS3_MAX_MASK if mask_only else NMS3_MAX_VALUES)
+    return out
+
+
+def _nms3d_minmax_cuda(x):
+    mx = torch.empty(x.shape, device=x.device, dtype=torch.bool)
+    mn = torch.empty(x.shape, device=x.device, dtype=torch.bool)
+    _nms3d_call(x, mx, mn, NMS3_MINMAX)
+    return mx, mn
+
+
+_define("nms3d_fwd", "(Tensor x, bool mask_only) -> Tensor", _nms3d_cuda,
+        lambda x, mask_only: x.new_empty(x.shape, dtype=torch.bool if mask_only else x.dtype))
+_define("nms3d_minmax_fwd", "(Tensor x) -> (Tensor, Tensor)", _nms3d_minmax_cuda,
+        lambda x: (x.new_empty(x.shape, dtype=torch.bool), x.new_empty(x.shape, dtype=torch.bool)))
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -963,5 +1022,5 @@ OPERATORS: Tuple[str, ...] = (
     "warp_fwd", "warp_bwd", "warp_prelude", "warp_prelude_bwd", "remap_fwd", "remap_bwd", "filter2d_fwd", "filter2d_bwd_input",
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
-    "scale_octave_fwd",
+    "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd",
 )

@@ -16,6 +16,7 @@
 #include "ssim_vwalk.cuh"
 #include "corner_vwalk.cuh"
 #include "octave_vwalk.cuh"
+#include "nms.cuh"
 #include "gradient_tiled.cuh"
 
 namespace kb200 {
@@ -624,6 +625,30 @@ int kb200_scale_octave_forward(const void* x, const double* taps, const int* ksi
   if (rc == KB200_EUNSUPPORTED)
     set_error("the fused octave kernel is fp32 only, for the instantiated tap chains, with every tap count <= min(H, W) and rows that are a "
               "multiple of 4 floats (16-byte aligned), got L=%d H=%d W=%d", L, H, W);
+  return rc;
+}
+
+int kb200_nms2d_forward(const void* x, void* out, int B, int C, int H, int W, long long sB, long long sC, int k, int values, int dtype,
+                        void* stream) {
+  KB_CHECK_ARG(x && out, "null pointer argument");
+  KB_CHECK_ARG(B > 0 && C > 0 && H > 0 && W > 0, "bad sizes B=%d C=%d H=%d W=%d", B, C, H, W);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  const int rc = dtype == KB200_F32 ? nms2d_forward((const float*)x, out, B, C, H, W, sB, sC, k, values != 0, (cudaStream_t)stream)
+                                    : KB200_EUNSUPPORTED;
+  if (rc == KB200_EUNSUPPORTED)
+    set_error("the fused 2-D non-maximum suppression is fp32 only, for square odd kernel sizes 3..31, got k=%d", k);
+  return rc;
+}
+
+int kb200_nms3d_forward(const void* x, void* out0, void* out1, int B, int C, int L, int H, int W, long long sB, long long sC,
+                        long long sL, int mode, int dtype, void* stream) {
+  KB_CHECK_ARG(x && out0 && (mode != 2 || out1), "null pointer argument");
+  KB_CHECK_ARG(B > 0 && C > 0 && L > 0 && H > 0 && W > 0, "bad sizes B=%d C=%d L=%d H=%d W=%d", B, C, L, H, W);
+  KB_CHECK_ARG(mode >= 0 && mode <= 2, "bad mode %d", mode);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  const int rc = dtype == KB200_F32 ? nms3d_forward((const float*)x, out0, out1, B, C, L, H, W, sB, sC, sL, mode, (cudaStream_t)stream)
+                                    : KB200_EUNSUPPORTED;
+  if (rc == KB200_EUNSUPPORTED) set_error("the fused 3-D non-maximum suppression is fp32 only");
   return rc;
 }
 

@@ -16,6 +16,7 @@
 #include "../../kornia_b200/csrc/ssim_vwalk.cuh"
 #include "../../kornia_b200/csrc/corner_vwalk.cuh"
 #include "../../kornia_b200/csrc/octave_vwalk.cuh"
+#include "../../kornia_b200/csrc/nms.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -28,6 +29,7 @@ namespace kb200 {
 alignas(128) unsigned char sept_smem[256 * 1024];
 alignas(128) unsigned char f2d_smem[256 * 1024];
 alignas(128) unsigned char f2dt_smem[128 * 1024];
+alignas(128) unsigned char nms_smem[64 * 1024];
 alignas(128) unsigned char gradt_smem[256 * 1024];
 alignas(128) unsigned char ssimv_smem[256 * 1024];
 alignas(128) unsigned char corner_smem[256 * 1024];
@@ -503,6 +505,170 @@ static void test_octave_all() {
   test_octave_both<OctCopy6>(2, 83, 60, 9);
   test_octave_both<OctCopy5>(1, 21, 28, 1);
   test_octave_both<OctCopy5>(2, 140, 68, 11);
+}
+
+// ------------------------------------------------------------------------------------------ non-maximum suppression
+// Scalar restatement of kornia/geometry/subpix/nms.py: a position is kept when it is strictly greater than every
+// neighbour (explicit K = 3, 5, 7: in-image neighbours, the (K - 1) / 2 ring False; K >= 9: replicate-clamped neighbours
+// and 0, and False when the window holds a non-finite texel), in 3-D than its 26 neighbours (strictly smaller for the
+// minima), the border levels, rows and columns False.  Values are x * keep.  The source planes sit at a plane stride that
+// is not H * W (a permuted view), and texels are quantised to quarters so ties are common.
+static void nms_source(std::vector<float>& store, float*& x, size_t planes, size_t stride, size_t HW, int specials) {
+  x = aligned(store, planes * stride);
+  for (size_t i = 0; i < planes * stride; ++i) x[i] = (float)(rng() % 7) * 0.25f - 0.75f;
+  if (specials)
+    for (size_t p = 0; p < planes; ++p) special_texels(x + p * stride, HW, 1);
+}
+
+static void nms_bytes_as_float(const std::vector<unsigned char>& m, std::vector<float>& f) {
+  f.resize(m.size());
+  for (size_t i = 0; i < m.size(); ++i) f[i] = (float)m[i];
+}
+
+template <int K, bool VALUES>
+static void test_nms2d(int B, int C, int H, int W, int specials, unsigned grid) {
+  constexpr int R = K / 2;
+  const size_t HW = (size_t)H * W, planes = (size_t)B * C, stride = HW + 5;
+  std::vector<float> xs;
+  float* x;
+  nms_source(xs, x, planes, stride, HW, specials);
+  std::vector<float> want(planes * HW), got(planes * HW);
+  for (size_t pl = 0; pl < planes; ++pl)
+    for (int y = 0; y < H; ++y)
+      for (int xx = 0; xx < W; ++xx) {
+        const float* src = x + pl * stride;
+        const float c = src[(size_t)y * W + xx];
+        bool keep = K > 7 ? (bool)std::isfinite(c) && c > 0.f : y >= R && y < H - R && xx >= R && xx < W - R;
+        for (int dy = -R; dy <= R && keep; ++dy)
+          for (int dx = -R; dx <= R && keep; ++dx) {
+            const float n = src[(size_t)fold(y + dy, H, KB200_REPLICATE) * W + fold(xx + dx, W, KB200_REPLICATE)];
+            if (K > 7 && !std::isfinite(n)) keep = false;
+            else if ((dy || dx) && !(c > n)) keep = false;
+          }
+        want[pl * HW + (size_t)y * W + xx] = VALUES ? c * (keep ? 1.f : 0.f) : (float)keep;
+      }
+  Nms2dParams p{};
+  p.src = x;
+  p.sB = (long long)C * stride;
+  p.sC = (long long)stride;
+  p.C = C;
+  p.H = H;
+  p.W = W;
+  p.tiles_x = ceil_div(W, NMS_TW);
+  p.tiles_y = ceil_div(H, NMS_TH);
+  p.tiles = (long long)planes * p.tiles_x * p.tiles_y;
+  std::vector<float> os;
+  std::vector<unsigned char> om(planes * HW + 16, 0xff);
+  if (VALUES) {
+    p.out = aligned(os, planes * HW);
+  } else {
+    p.out = om.data();
+  }
+  emu::launch(grid, dim3(NMS_NT), [&] { nms2d_kernel<K, VALUES>(p); });
+  if (VALUES) std::copy((float*)p.out, (float*)p.out + planes * HW, got.begin());
+  else nms_bytes_as_float(std::vector<unsigned char>(om.begin(), om.begin() + planes * HW), got);
+  compare_bits_or_nan("nms2d_kernel K=" + std::to_string(K) + (VALUES ? " values " : " mask ") + std::to_string(B) + "x" + std::to_string(C) + "x" +
+                          std::to_string(H) + "x" + std::to_string(W) + (specials ? " special texels" : "") + " grid=" + std::to_string(grid),
+                      got.data(), want.data(), planes * HW);
+}
+
+template <int MODE>
+static void test_nms3d(int B, int C, int L, int H, int W, int specials, unsigned grid) {
+  const size_t HW = (size_t)H * W, vols = (size_t)B * C, lstride = HW + 3, n = vols * L * HW;
+  std::vector<float> xs;
+  float* x;
+  nms_source(xs, x, vols * L, lstride, HW, specials);
+  // (B, L, C, H, W) storage read as (B, C, L, H, W): the permuted view ScaleSpaceDetector hands over
+  const long long sC = (long long)lstride, sL = (long long)C * lstride, sB = (long long)L * C * lstride;
+  std::vector<float> wmax(n), wmin(n), got(n);
+  for (size_t v = 0; v < vols; ++v) {
+    const float* src = x + (v / C) * sB + (v % C) * sC;
+    for (int l = 0; l < L; ++l)
+      for (int y = 0; y < H; ++y)
+        for (int xx = 0; xx < W; ++xx) {
+          const float c = src[l * sL + (size_t)y * W + xx];
+          bool kmax = l >= 1 && l < L - 1 && y >= 1 && y < H - 1 && xx >= 1 && xx < W - 1, kmin = kmax;
+          for (int dl = -1; dl <= 1 && (kmax || kmin); ++dl)
+            for (int dy = -1; dy <= 1; ++dy)
+              for (int dx = -1; dx <= 1; ++dx) {
+                if (!dl && !dy && !dx) continue;
+                const float nb = src[(l + dl) * sL + (size_t)(y + dy) * W + xx + dx];
+                kmax = kmax && c > nb;
+                kmin = kmin && c < nb;
+              }
+          const size_t o = ((v * L + l) * H + y) * W + xx;
+          wmax[o] = MODE == NMS3_MAX_VALUES ? c * (kmax ? 1.f : 0.f) : (float)kmax;
+          wmin[o] = (float)kmin;
+        }
+  }
+  Nms3dParams p{};
+  p.src = x;
+  p.sB = sB;
+  p.sC = sC;
+  p.sL = sL;
+  p.C = C;
+  p.L = L;
+  p.H = H;
+  p.W = W;
+  p.tiles_x = ceil_div(W, NMS3_TW);
+  p.tiles_y = ceil_div(H, NMS3_TH);
+  p.tiles = (long long)vols * p.tiles_x * p.tiles_y;
+  std::vector<float> os;
+  std::vector<unsigned char> o0(n, 0xff), o1(n, 0xff);
+  p.out0 = MODE == NMS3_MAX_VALUES ? (void*)aligned(os, n) : (void*)o0.data();
+  p.out1 = o1.data();
+  emu::launch(grid, dim3(NMS3_NT), [&] { nms3d_kernel<MODE>(p); });
+  const std::string what = std::string("nms3d_kernel ") + (MODE == NMS3_MAX_MASK ? "mask " : MODE == NMS3_MAX_VALUES ? "values " : "minmax ") +
+                           std::to_string(B) + "x" + std::to_string(C) + "x" + std::to_string(L) + "x" + std::to_string(H) + "x" + std::to_string(W) +
+                           (specials ? " special texels" : "") + " grid=" + std::to_string(grid);
+  if (MODE == NMS3_MAX_VALUES) std::copy((float*)p.out0, (float*)p.out0 + n, got.begin());
+  else nms_bytes_as_float(o0, got);
+  compare_bits_or_nan(what + (MODE == NMS3_MINMAX ? " (maxima)" : ""), got.data(), wmax.data(), n);
+  if (MODE == NMS3_MINMAX) {
+    nms_bytes_as_float(o1, got);
+    compare_bits_or_nan(what + " (minima)", got.data(), wmin.data(), n);
+  }
+}
+
+template <int K>
+static void test_nms2d_both(int B, int C, int H, int W, int specials, unsigned grid) {
+  test_nms2d<K, false>(B, C, H, W, specials, grid);
+  test_nms2d<K, true>(B, C, H, W, specials, grid);
+}
+
+// The fixed list (also alone: run_emu --nms): every instantiated K in both forms on a shape with partial edge tiles;
+// tiles that lie wholly inside the halo (H or W below K, 1 x 1, 2 x 2); grids that do not divide the tiles; and the 3-D
+// kernel in all three modes on odd widths, level counts 1, 2, 3 and 5, with finite and special texels.
+static void test_nms_all() {
+  test_nms2d_both<3>(1, 2, 70, 131, 1, 5);
+  test_nms2d_both<5>(2, 1, 33, 67, 0, 3);
+  test_nms2d_both<7>(1, 1, 40, 130, 1, 2);
+  test_nms2d_both<9>(1, 2, 45, 70, 1, 4);
+  test_nms2d_both<11>(1, 1, 33, 65, 0, 1);
+  test_nms2d_both<13>(1, 1, 36, 66, 1, 2);
+  test_nms2d_both<15>(2, 1, 61, 68, 1, 3);
+  test_nms2d_both<17>(1, 1, 20, 70, 0, 2);
+  test_nms2d_both<19>(1, 1, 34, 40, 1, 1);
+  test_nms2d_both<21>(1, 1, 30, 15, 1, 2);
+  test_nms2d_both<23>(1, 1, 40, 65, 0, 2);
+  test_nms2d_both<25>(1, 1, 33, 30, 1, 1);
+  test_nms2d_both<27>(1, 1, 26, 80, 0, 2);
+  test_nms2d_both<29>(1, 1, 35, 66, 1, 2);
+  test_nms2d_both<31>(1, 2, 40, 70, 1, 3);
+  test_nms2d_both<7>(1, 1, 5, 3, 1, 1);
+  test_nms2d_both<15>(1, 1, 9, 6, 1, 1);
+  test_nms2d_both<3>(2, 1, 1, 1, 0, 1);
+  test_nms2d_both<9>(1, 1, 1, 1, 1, 1);
+  test_nms2d_both<5>(1, 1, 2, 2, 0, 1);
+  test_nms2d_both<31>(1, 1, 2, 2, 1, 1);
+  for (int sp = 0; sp < 2; ++sp) {
+    test_nms3d<NMS3_MINMAX>(1, 2, 5, 19, 131, sp, 3);
+    test_nms3d<NMS3_MAX_MASK>(2, 1, 3, 9, 30, sp, 2);
+    test_nms3d<NMS3_MAX_VALUES>(1, 1, 4, 17, 15, sp, 1);
+    test_nms3d<NMS3_MINMAX>(1, 1, 2, 5, 5, sp, 1);
+    test_nms3d<NMS3_MINMAX>(1, 1, 1, 1, 1, sp, 1);
+    test_nms3d<NMS3_MAX_VALUES>(1, 2, 3, 3, 3, sp, 2);
+  }
 }
 
 // ------------------------------------------------------------------------------------------ feature responses
@@ -1235,6 +1401,8 @@ static void fuzz(int rounds) {
   auto pick = [&](int lo, int hi) { return lo + (int)(g() % (unsigned)(hi - lo + 1)); };
   std::mt19937 go(20261017);  // the octave cases draw from their own stream, so the other cases stay what they were
   auto opick = [&](int lo, int hi) { return lo + (int)(go() % (unsigned)(hi - lo + 1)); };
+  std::mt19937 gn(20261018);  // and the non-maximum-suppression cases from theirs
+  auto npick = [&](int lo, int hi) { return lo + (int)(gn() % (unsigned)(hi - lo + 1)); };
   for (int r = 0; r < rounds; ++r) {
     if (r % 10 == 9) {  // ScalePyramid octave: any chain, both stage-0 modes, sides from the largest tap count up, any grid
       const int which = opick(0, 4), planes = opick(1, 2), sp = opick(0, 2);
@@ -1246,6 +1414,22 @@ static void fuzz(int rounds) {
       else if (which == 2) test_octave<OctDouble>(planes, H, W, sp, grid);
       else if (which == 3) test_octave<OctCopy6>(planes, H, W, sp, grid);
       else test_octave<OctCopy5>(planes, H, W, sp, grid);
+    }
+    if (r % 10 == 4) {  // non-maximum suppression: any K and form, any shape (odd widths, sides below K), 3-D modes, any grid
+      const int H = npick(1, 80), W = npick(1, 140), sp = npick(0, 1);
+      const unsigned grid = (unsigned)npick(1, 9);
+      switch (npick(0, 9)) {
+        case 0: test_nms2d_both<3>(npick(1, 2), npick(1, 2), H, W, sp, grid); break;
+        case 1: test_nms2d_both<5>(1, npick(1, 2), H, W, sp, grid); break;
+        case 2: test_nms2d_both<7>(1, 1, H, W, sp, grid); break;
+        case 3: test_nms2d_both<9>(1, npick(1, 2), H, W, sp, grid); break;
+        case 4: test_nms2d_both<15>(npick(1, 2), 1, H, W, sp, grid); break;
+        case 5: test_nms2d_both<21>(1, 1, H, W, sp, grid); break;
+        case 6: test_nms2d_both<31>(1, 1, H, W, sp, grid); break;
+        case 7: test_nms3d<NMS3_MAX_MASK>(npick(1, 2), npick(1, 2), npick(1, 5), H / 2 + 1, W, sp, grid); break;
+        case 8: test_nms3d<NMS3_MAX_VALUES>(1, npick(1, 2), npick(1, 5), H / 2 + 1, W, sp, grid); break;
+        default: test_nms3d<NMS3_MINMAX>(npick(1, 2), npick(1, 2), npick(1, 6), H / 2 + 1, W, sp, grid); break;
+      }
     }
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
@@ -1358,6 +1542,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--octave") {
     test_octave_all();
     printf("%s: %d failing comparisons (ScalePyramid octave, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--nms") {
+    test_nms_all();
+    printf("%s: %d failing comparisons (non-maximum suppression, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {

@@ -83,5 +83,15 @@ for shape in ((3, 100, 192, 3), (2, 70, 132, 1), (1, 33, 45, 3)):  # the last on
     KC.undistort_image_from_uint8(frames, camq, torch.tensor([[-0.2, 0.05, 0.001, -0.002, 0.01]], device=dev).expand(shape[0], 5).contiguous())
 # ScalePyramid: the octave kernel (blur and copy stages, a band of 4 columns, more CTAs than bands), tiny octaves composed
 KT.ScalePyramid(min_size=8)(torch.rand(2, 1, 100, 132, generator=g).to(dev))
+# non-maximum suppression: the 2-D kernel in both forms (explicit 5 x 5 and general 15 x 15, odd width, partial tiles), the
+# 3-D kernel on a permuted (B, C, L, H, W) view in both nms3d forms and as nms3d_minmax
+KG = K.geometry
+resp = torch.rand(2, 2, 70, 133, generator=g).to(dev)
+KG.nms2d(resp, (5, 5), True)
+KG.NonMaximaSuppression2d((15, 15)).to(dev)(resp)
+octv = torch.rand(1, 5, 2, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4)
+KG.nms3d(octv, (3, 3, 3), True)
+KG.nms3d(octv, (3, 3, 3))
+KG.nms3d_minmax(octv)
 torch.cuda.synchronize()
 print("sanitize workload done")
