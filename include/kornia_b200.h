@@ -284,6 +284,24 @@ int kb200_nms3d_forward(const void* x, void* out0, void* out1, int B, int C, int
                         long long sL, int mode, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Sub-pixel refinement of 3-D scale-space maxima (conv_quad_interp3d / iterative_quad_interp3d of
+ * geometry/subpix/spatial_soft_argmax.py) in ONE kernel per call: 4 B read (5 B with a mask) and 16 B written per element,
+ * with no host synchronisation, instead of a nonzero, index gathers and tens of small kernels per iteration.
+ *   x       fp32 (B, C, L, H, W) whose H x W planes are dense; sB, sC, sL are its element strides, so a permuted
+ *           (B, C, L, H, W) view is read in place
+ *   mask    contiguous bool (B, C, L, H, W) NMS mask, or NULL: nms3d(x, (3, 3, 3), True) is computed in the kernel
+ *   coords  contiguous (B, C, 3, L, H, W) [level, x, y]: the grid, refined at the maxima
+ *   y       (B, C, L, H, W) at the element strides ysB .. ysW (those of x.clone()): x, refined at the maxima
+ *   radius  the conv form's dilation radius (>= 1), or 0 for the iterative form
+ *   max_shift, bonus  the Python floats rounded to fp32; add_bonus = (strict_maxima_bonus > 0)
+ * L, H or W < 3 writes the grid and the copy only, as the reference returns them.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_quad_interp3d_forward(const void* x, const void* mask, void* coords, void* y, int B, int C, int L, int H, int W, long long sB,
+                                long long sC, long long sL, long long ysB, long long ysC, long long ysL, long long ysH,
+                                long long ysW, int n_iters, int radius, float max_shift, float bonus, int add_bonus, int allow_scale,
+                                int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

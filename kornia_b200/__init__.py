@@ -24,10 +24,12 @@ def install(kornia_module=None) -> None:
     ``get_motion_kernel2d``, whose kernel must be built on the GPU, and the ``harris_response`` / ``gftt_response`` /
     ``hessian_response`` of the classical detectors, the ``ScalePyramid`` class their scale-space detectors build, and the
     non-maximum suppression ``nms2d`` / ``nms3d`` / ``nms3d_minmax`` / ``NonMaximaSuppression2d`` /
-    ``NonMaximaSuppression3d`` of the detectors and the sub-pixel refiners) on an imported ``kornia`` package.  A defining
-    module the package lacks, or a name its module does not define, is skipped.  Rebinding a class affects modules
-    constructed afterwards: a ``ScaleSpaceDetector`` or ``MultiResolutionDetector`` built before ``install()`` keeps the
-    reference pyramid and the reference ``NonMaximaSuppression2d`` it holds.
+    ``NonMaximaSuppression3d`` of the detectors and the sub-pixel refiners, and those refiners ``conv_quad_interp3d`` /
+    ``iterative_quad_interp3d`` / ``ConvQuadInterp3d`` / ``IterativeQuadInterp3d`` / ``AdaptiveQuadInterp3d``) on an
+    imported ``kornia`` package.  A defining module the package lacks, or a name its module does not define, is skipped.
+    Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``, ``MultiResolutionDetector`` or
+    ``SIFTFeatureScaleSpace`` built before ``install()`` keeps the reference pyramid, the reference
+    ``NonMaximaSuppression2d`` and the reference sub-pixel refiner it holds.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -69,6 +71,13 @@ def install(kornia_module=None) -> None:
         "nms3d_minmax": ("geometry.subpix.nms", geometry.subpix.nms3d_minmax),
         "NonMaximaSuppression2d": ("geometry.subpix.nms", geometry.subpix.NonMaximaSuppression2d),
         "NonMaximaSuppression3d": ("geometry.subpix.nms", geometry.subpix.NonMaximaSuppression3d),
+        # ScaleSpaceDetector builds its default AdaptiveQuadInterp3d (and checks isinstance against all three classes, so
+        # its precomputed NMS masks are still passed) and SIFTFeatureScaleSpace its ConvQuadInterp3d from these names
+        "conv_quad_interp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.conv_quad_interp3d),
+        "iterative_quad_interp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.iterative_quad_interp3d),
+        "ConvQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.ConvQuadInterp3d),
+        "IterativeQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.IterativeQuadInterp3d),
+        "AdaptiveQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.AdaptiveQuadInterp3d),
     }
     originals = {}
     for name, (mod, fn) in defining.items():

@@ -845,6 +845,30 @@ _define("nms3d_minmax_fwd", "(Tensor x) -> (Tensor, Tensor)", _nms3d_minmax_cuda
         lambda x: (x.new_empty(x.shape, dtype=torch.bool), x.new_empty(x.shape, dtype=torch.bool)))
 
 
+def _quad_interp3d_cuda(x, mask, n_iters, max_subpixel_shift, strict_maxima_bonus, dilation_radius, allow_scale_steps):
+    """coords (B, C, 3, D, H, W) and y (the strides of x.clone()); ``dilation_radius`` 0 is the iterative form."""
+    _require_cuda(x, "input")
+    B, C, D, H, W = x.shape
+    coords = torch.empty((B, C, 3, D, H, W), device=x.device, dtype=x.dtype)
+    y = torch.empty_like(x)
+    if x.numel() == 0:
+        return coords, y
+    xs = _dense_planes(x)
+    radius = min(dilation_radius, max(D, H, W))  # a radius past the largest side reaches every voxel either way
+    with torch.cuda.device(x.device), _Timed("quad_interp3d_forward", x):
+        _lib.call("kb200_quad_interp3d_forward", _ptr(xs), _ptr(mask), _ptr(coords), _ptr(y), B, C, D, H, W, xs.stride(0), xs.stride(1),
+                  xs.stride(2), *y.stride(), n_iters, radius, max_subpixel_shift, strict_maxima_bonus, strict_maxima_bonus > 0,
+                  allow_scale_steps, _dtype_code(x), _stream(x))
+    _bump()
+    return coords, y
+
+
+_define("quad_interp3d_fwd",
+        "(Tensor x, Tensor? mask, int n_iters, float max_subpixel_shift, float strict_maxima_bonus, int dilation_radius, "
+        "bool allow_scale_steps) -> (Tensor, Tensor)", _quad_interp3d_cuda,
+        lambda x, mask, *_: (x.new_empty((x.shape[0], x.shape[1], 3) + tuple(x.shape[2:])), torch.empty_like(x)))
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -1022,5 +1046,5 @@ OPERATORS: Tuple[str, ...] = (
     "warp_fwd", "warp_bwd", "warp_prelude", "warp_prelude_bwd", "remap_fwd", "remap_bwd", "filter2d_fwd", "filter2d_bwd_input",
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
-    "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd",
+    "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd", "quad_interp3d_fwd",
 )

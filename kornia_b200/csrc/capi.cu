@@ -17,6 +17,7 @@
 #include "corner_vwalk.cuh"
 #include "octave_vwalk.cuh"
 #include "nms.cuh"
+#include "quad_interp.cuh"
 #include "gradient_tiled.cuh"
 
 namespace kb200 {
@@ -650,6 +651,22 @@ int kb200_nms3d_forward(const void* x, void* out0, void* out1, int B, int C, int
                                     : KB200_EUNSUPPORTED;
   if (rc == KB200_EUNSUPPORTED) set_error("the fused 3-D non-maximum suppression is fp32 only");
   return rc;
+}
+
+int kb200_quad_interp3d_forward(const void* x, const void* mask, void* coords, void* y, int B, int C, int L, int H, int W, long long sB,
+                                long long sC, long long sL, long long ysB, long long ysC, long long ysL, long long ysH,
+                                long long ysW, int n_iters, int radius, float max_shift, float bonus, int add_bonus, int allow_scale,
+                                int dtype, void* stream) {
+  KB_CHECK_ARG(x && coords && y, "null pointer argument");
+  KB_CHECK_ARG(B > 0 && C > 0 && L > 0 && H > 0 && W > 0, "bad sizes B=%d C=%d L=%d H=%d W=%d", B, C, L, H, W);
+  KB_CHECK_ARG(radius >= 0, "bad dilation radius %d", radius);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused sub-pixel refinement is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  return quad_interp3d_forward((const float*)x, (const unsigned char*)mask, (float*)coords, (float*)y, B, C, L, H, W, sB, sC, sL, ysB,
+                               ysC, ysL, ysH, ysW, n_iters, radius, max_shift, bonus, add_bonus, allow_scale, (cudaStream_t)stream);
 }
 
 int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void* kernel_y, void* out, int B, int C, int H, int W,

@@ -175,10 +175,55 @@ __global__ void __launch_bounds__(NMS_NT) nms2d_kernel(const Nms2dParams p) {
   }
 }
 
-template <int MODE>
-__global__ void __launch_bounds__(NMS3_NT) nms3d_kernel(const Nms3dParams p) {
-  constexpr bool MINMAX = MODE == NMS3_MINMAX, VALUES = MODE == NMS3_MAX_VALUES;
+// One level of the 3-D walk: stage the 128 x 8 tile at (x0, y0) of the dense H x W plane `lev` plus a one-texel halo,
+// replicate-clamped, in `s`; then reduce this thread's 4 columns (c4, row ry): the centre values, the 3 x 3 max and the
+// 8-neighbour max (and with MIN the same minima).  Shared by nms3d_kernel and the sub-pixel refinement kernel
+// (quad_interp.cuh), which computes its NMS mask on the same walk.
+template <bool MIN>
+__device__ __forceinline__ void nms3_stage_level(float* s, const float* lev, int H, int W, int x0, int y0, int tid, int c4, int ry,
+                                                 float nval[4], float nmax[4], float n8max[4], float nmin[4], float n8min[4]) {
   constexpr int SW = NMS3_TW + 2, SH = NMS3_TH + 2;
+  __syncthreads();  // the previous level's readers are done with shared memory
+  for (int i = tid; i < SH * SW; i += NMS3_NT) {
+    const int ly = i / SW, lx = i - ly * SW;
+    const int yy = min(max(y0 - 1 + ly, 0), H - 1), xx = min(max(x0 - 1 + lx, 0), W - 1);
+    s[i] = ldg(lev + (long long)yy * W + xx);
+  }
+  __syncthreads();
+  float vmax[6], vmin[6], top[4], bot[4];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    const float a = s[ry * SW + c4 + j], b = s[(ry + 1) * SW + c4 + j], d = s[(ry + 2) * SW + c4 + j];
+    vmax[j] = nan_max(nan_max(a, b), d);
+    vmin[j] = nan_min(nan_min(a, b), d);
+    if (j >= 1 && j <= 4) {
+      top[j - 1] = a;
+      bot[j - 1] = d;
+      nval[j - 1] = b;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float side_max = nan_max(vmax[i], vmax[i + 2]), side_min = nan_min(vmin[i], vmin[i + 2]);
+    nmax[i] = nan_max(side_max, vmax[i + 1]);
+    n8max[i] = nan_max(side_max, nan_max(top[i], bot[i]));
+    if (MIN) {
+      nmin[i] = nan_min(side_min, vmin[i + 1]);
+      n8min[i] = nan_min(side_min, nan_min(top[i], bot[i]));
+    }
+  }
+}
+
+// The 26-neighbour test of the ring's middle level: its centre against the 3 x 3 max of the levels either side and its
+// own 8-neighbour max.
+__device__ __forceinline__ bool nms3_is_max(float c, float below_max, float c8max, float above_max) {
+  return c > nan_max(nan_max(below_max, c8max), above_max);
+}
+
+// 4 CTAs per SM: without the bound ptxas gives the minmax form 79 registers and 3 CTAs
+template <int MODE>
+__global__ void __launch_bounds__(NMS3_NT, 4) nms3d_kernel(const Nms3dParams p) {
+  constexpr bool MINMAX = MODE == NMS3_MINMAX, VALUES = MODE == NMS3_MAX_VALUES;
   extern __shared__ __align__(128) unsigned char nms_smem[];
   float* s = reinterpret_cast<float*>(nms_smem);
   const int tid = threadIdx.x;
@@ -197,43 +242,14 @@ __global__ void __launch_bounds__(NMS3_NT) nms3d_kernel(const Nms3dParams p) {
     float pmax[4] = {}, pmin[4] = {}, cmax[4] = {}, cmin[4] = {}, c8max[4] = {}, c8min[4] = {}, cval[4] = {};
     for (int l = 0; l <= p.L; ++l) {
       float nmax[4] = {}, nmin[4] = {}, n8max[4] = {}, n8min[4] = {}, nval[4] = {};
-      if (l < p.L) {
-        const float* lev = src + (long long)l * p.sL;
-        __syncthreads();  // the previous level's readers are done with shared memory
-        for (int i = tid; i < SH * SW; i += NMS3_NT) {
-          const int ly = i / SW, lx = i - ly * SW;
-          const int yy = min(max(y0 - 1 + ly, 0), p.H - 1), xx = min(max(x0 - 1 + lx, 0), p.W - 1);
-          s[i] = ldg(lev + (long long)yy * p.W + xx);
-        }
-        __syncthreads();
-        float vmax[6], vmin[6], top[4], bot[4];
-#pragma unroll
-        for (int j = 0; j < 6; ++j) {
-          const float a = s[ry * SW + c4 + j], b = s[(ry + 1) * SW + c4 + j], d = s[(ry + 2) * SW + c4 + j];
-          vmax[j] = nan_max(nan_max(a, b), d);
-          vmin[j] = nan_min(nan_min(a, b), d);
-          if (j >= 1 && j <= 4) {
-            top[j - 1] = a;
-            bot[j - 1] = d;
-            nval[j - 1] = b;
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float side_max = nan_max(vmax[i], vmax[i + 2]), side_min = nan_min(vmin[i], vmin[i + 2]);
-          nmax[i] = nan_max(side_max, vmax[i + 1]);
-          nmin[i] = nan_min(side_min, vmin[i + 1]);
-          n8max[i] = nan_max(side_max, nan_max(top[i], bot[i]));
-          n8min[i] = nan_min(side_min, nan_min(top[i], bot[i]));
-        }
-      }
+      if (l < p.L) nms3_stage_level<MINMAX>(s, src + (long long)l * p.sL, p.H, p.W, x0, y0, tid, c4, ry, nval, nmax, n8max, nmin, n8min);
       if (l >= 1 && active) {  // level l - 1 is complete: False on the border levels (l - 1 == 0 or l == L)
         const bool level_in = l >= 2 && l < p.L && row_in;
         bool kmax[4], kmin[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const bool in = level_in && gx + i >= 1 && gx + i < p.W - 1;
-          kmax[i] = in && cval[i] > nan_max(nan_max(pmax[i], c8max[i]), nmax[i]);
+          kmax[i] = in && nms3_is_max(cval[i], pmax[i], c8max[i], nmax[i]);
           kmin[i] = in && cval[i] < nan_min(nan_min(pmin[i], c8min[i]), nmin[i]);
         }
         const long long off = (((long long)vol * p.L + (l - 1)) * p.H + gy) * p.W + gx;

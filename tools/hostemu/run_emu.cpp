@@ -17,6 +17,7 @@
 #include "../../kornia_b200/csrc/corner_vwalk.cuh"
 #include "../../kornia_b200/csrc/octave_vwalk.cuh"
 #include "../../kornia_b200/csrc/nms.cuh"
+#include "../../kornia_b200/csrc/quad_interp.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -668,6 +669,157 @@ static void test_nms_all() {
     test_nms3d<NMS3_MINMAX>(1, 1, 2, 5, 5, sp, 1);
     test_nms3d<NMS3_MINMAX>(1, 1, 1, 1, 1, sp, 1);
     test_nms3d<NMS3_MAX_VALUES>(1, 2, 3, 3, 3, sp, 2);
+  }
+}
+
+// ------------------------------------------------------------------------------------------ sub-pixel refinement
+// Scalar restatement of conv_quad_interp3d / iterative_quad_interp3d (kornia/geometry/subpix/spatial_soft_argmax.py):
+// every maximum (the given mask, or strictly above its 26 neighbours with the border False) runs all n_iters iterations
+// (a failed keypoint is frozen), solving the 3 x 3 x 3 fit at its clamped position in the reference's operation order;
+// the conv form also needs a mask voxel within L-inf `radius`.  The source is a permuted (B, L, C, H, W) store read as
+// (B, C, L, H, W), texels are normal draws (keypoints walk) or special values.
+static void test_quad(int B, int C, int L, int H, int W, int radius, bool has_mask, int n_iters, float shift, float bonus, bool allow,
+                      int specials, unsigned grid) {
+  const size_t HW = (size_t)H * W, vols = (size_t)B * C, lstride = HW + 3, n = vols * L * HW;
+  std::vector<float> xs;
+  float* x = aligned(xs, vols * L * lstride);
+  std::normal_distribution<float> nd(0.f, 1.f);
+  for (size_t i = 0; i < vols * L * lstride; ++i) x[i] = nd(rng);
+  if (specials)
+    for (size_t p = 0; p < vols * L; ++p) special_texels(x + p * lstride, HW, 1);
+  const long long sC = (long long)lstride, sL = (long long)C * lstride, sB = (long long)L * C * lstride;
+  std::vector<unsigned char> mask(n, 0);
+  for (size_t i = 0; i < n; ++i) mask[i] = rng() % 25 == 0 || (i / W) % H == 0;  // sparse, and every first row
+  auto src = [&](size_t v, int d, int h, int w) { return x[(v / C) * sB + (v % C) * sC + d * sL + (size_t)h * W + w]; };
+  auto is_max = [&](size_t v, int d, int h, int w) {
+    if (has_mask) return mask[((v * L + d) * H + h) * W + w] != 0;
+    if (d < 1 || d > L - 2 || h < 1 || h > H - 2 || w < 1 || w > W - 2) return false;
+    const float c = src(v, d, h, w);
+    bool k = true;
+    for (int a = -1; a <= 1; ++a)
+      for (int b = -1; b <= 1; ++b)
+        for (int e = -1; e <= 1; ++e)
+          if ((a || b || e) && !(c > src(v, d + a, h + b, w + e))) k = false;
+    return k;
+  };
+  std::vector<float> wc(3 * n), wy(n);
+  const bool refine = L >= 3 && H >= 3 && W >= 3;
+  for (size_t v = 0; v < vols; ++v)
+    for (int d0 = 0; d0 < L; ++d0)
+      for (int h0 = 0; h0 < H; ++h0)
+        for (int w0 = 0; w0 < W; ++w0) {
+          const size_t o = ((v * L + d0) * H + h0) * W + w0, co = ((v * 3 * L + d0) * H + h0) * W + w0;
+          float cs = (float)d0, cx = (float)w0, cy = (float)h0, y = src(v, d0, h0, w0);
+          if (refine && is_max(v, d0, h0, w0)) {
+            int d = d0, h = h0, w = w0;
+            bool valid = true;
+            float s[3] = {0.f, 0.f, 0.f}, gds = 0.f;  // x, y, level
+            for (int it = 0; it < n_iters; ++it) {
+              if (!valid) continue;
+              const int dc = std::min(std::max(d, 1), L - 2), hc = std::min(std::max(h, 1), H - 2), wc_ = std::min(std::max(w, 1), W - 2);
+              auto P = [&](int a, int b, int e) { return src(v, dc + a, hc + b, wc_ + e); };
+              const float g[3] = {0.5f * (P(0, 0, 1) - P(0, 0, -1)), 0.5f * (P(0, 1, 0) - P(0, -1, 0)), 0.5f * (P(1, 0, 0) - P(-1, 0, 0))};
+              const float c2 = 2.f * P(0, 0, 0);
+              const float dxx = P(0, 0, 1) - c2 + P(0, 0, -1), dyy = P(0, 1, 0) - c2 + P(0, -1, 0), dss = P(1, 0, 0) - c2 + P(-1, 0, 0);
+              const float dxy = 0.25f * (P(0, 1, 1) - P(0, 1, -1) - P(0, -1, 1) + P(0, -1, -1));
+              const float dxs = 0.25f * (P(1, 0, 1) - P(1, 0, -1) - P(-1, 0, 1) + P(-1, 0, -1));
+              const float dys = 0.25f * (P(1, 1, 0) - P(1, -1, 0) - P(-1, 1, 0) + P(-1, -1, 0));
+              const float r0 = -g[0], r1 = -g[1], r2 = -g[2];
+              const float m00 = dyy * dss - dys * dys, m01 = dxy * dss - dys * dxs, m02 = dxy * dys - dyy * dxs;
+              const float det = dxx * m00 - dxy * m01 + dxs * m02;
+              bool ok = std::fabs(det) > 1e-7f;
+              const float sd = ok ? det : 1.f;
+              const float sn[3] = {(r0 * m00 - dxy * (r1 * dss - dys * r2) + dxs * (r1 * dys - dyy * r2)) / sd,
+                                   (dxx * (r1 * dss - dys * r2) - r0 * m01 + dxs * (dxy * r2 - r1 * dxs)) / sd,
+                                   (dxx * (dyy * r2 - r1 * dys) - dxy * (dxy * r2 - r1 * dxs) + r0 * m02) / sd};
+              if (radius > 0) {
+                bool near = false;
+                for (int a = std::max(dc - radius, 0); a <= std::min(dc + radius, L - 1); ++a)
+                  for (int b = std::max(hc - radius, 0); b <= std::min(hc + radius, H - 1); ++b)
+                    for (int e = std::max(wc_ - radius, 0); e <= std::min(wc_ + radius, W - 1); ++e) near = near || is_max(v, a, b, e);
+                ok = ok && near;
+              }
+              valid = ok;
+              if (!valid) continue;
+              for (int k = 0; k < 3; ++k) s[k] = sn[k];
+              gds = g[0] * sn[0] + g[1] * sn[1] + g[2] * sn[2];
+              int* pos[3] = {&w, &h, &d};
+              const int size[3] = {W, H, L};
+              for (int k = 0; k < (allow ? 3 : 2) && valid; ++k) {
+                const int nw = *pos[k] + (sn[k] > shift) - (sn[k] < -shift);
+                valid = nw >= 1 && nw <= size[k] - 2;
+                *pos[k] = std::min(std::max(nw, 0), size[k] - 1);
+              }
+            }
+            valid = valid && std::fabs(s[0]) <= 1.5f && std::fabs(s[1]) <= 1.5f && std::fabs(s[2]) <= 1.5f;
+            if (valid) {
+              cs = (float)d + s[2];
+              cx = (float)w + s[0];
+              cy = (float)h + s[1];
+            }
+            y = src(v, d, h, w) + 0.5f * (valid ? gds : 0.f);
+            if (bonus > 0.f) y = y + bonus * (valid ? 1.f : 0.f);
+          }
+          wc[co] = cs;
+          wc[co + L * HW] = cx;
+          wc[co + 2 * L * HW] = cy;
+          wy[o] = y;
+        }
+  QuadParams p{};
+  p.src = x;
+  p.mask = has_mask ? mask.data() : nullptr;
+  std::vector<float> cstore, ystore;
+  p.coords = aligned(cstore, 3 * n);
+  p.y = aligned(ystore, n);
+  std::fill(p.coords, p.coords + 3 * n, std::nanf(""));
+  std::fill(p.y, p.y + n, std::nanf(""));
+  p.sB = sB;
+  p.sC = sC;
+  p.sL = sL;
+  p.ysW = 1;
+  p.ysH = W;
+  p.ysL = (long long)HW;
+  p.ysC = (long long)L * HW;
+  p.ysB = (long long)C * L * HW;
+  p.C = C;
+  p.L = L;
+  p.H = H;
+  p.W = W;
+  p.tiles_x = ceil_div(W, NMS3_TW);
+  p.tiles_y = ceil_div(H, NMS3_TH);
+  p.tiles = (long long)vols * p.tiles_x * p.tiles_y;
+  p.n_iters = n_iters;
+  p.radius = radius;
+  p.max_shift = shift;
+  p.bonus = bonus;
+  p.add_bonus = bonus > 0.f;
+  p.allow_scale = allow;
+  p.refine = refine;
+  if (has_mask && radius > 0) emu::launch(grid, dim3(NMS3_NT), [&] { quad_interp3d_kernel<true, true>(p); });
+  else if (has_mask) emu::launch(grid, dim3(NMS3_NT), [&] { quad_interp3d_kernel<true, false>(p); });
+  else if (radius > 0) emu::launch(grid, dim3(NMS3_NT), [&] { quad_interp3d_kernel<false, true>(p); });
+  else emu::launch(grid, dim3(NMS3_NT), [&] { quad_interp3d_kernel<false, false>(p); });
+  const std::string what = std::string("quad_interp3d_kernel ") + (radius ? "conv r=" + std::to_string(radius) : std::string("iterative")) +
+                           (has_mask ? " mask " : " nms ") + std::to_string(B) + "x" + std::to_string(C) + "x" + std::to_string(L) + "x" +
+                           std::to_string(H) + "x" + std::to_string(W) + " n_iters=" + std::to_string(n_iters) + " shift=" + std::to_string(shift) +
+                           (allow ? "" : " flat") + (specials ? " special texels" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what + " (coords)", p.coords, wc.data(), 3 * n);
+  compare_bits_or_nan(what + " (y)", p.y, wy.data(), n);
+}
+
+// The fixed list (also alone: run_emu --quad): both forms, with and without a mask, radii 1 and 2, n_iters 0, 1 and 5,
+// both thresholds and allow_scale_steps, partial edge tiles, D / H / W below 3, special texels, grids that do not divide.
+static void test_quad_all() {
+  for (int sp = 0; sp < 2; ++sp) {
+    test_quad(1, 2, 5, 19, 131, 1, false, 5, 0.6f, 10.f, true, sp, 3);
+    test_quad(1, 1, 5, 17, 30, 2, true, 5, 0.3f, 0.f, true, sp, 2);
+    test_quad(2, 1, 4, 9, 21, 0, false, 5, 0.3f, 10.f, false, sp, 1);
+    test_quad(1, 2, 6, 12, 15, 0, true, 1, 0.6f, 0.f, true, sp, 4);
+    test_quad(1, 1, 5, 16, 20, 1, true, 0, 0.3f, 10.f, true, sp, 1);
+    test_quad(1, 1, 4, 11, 13, 1, false, 5, 0.3f, 10.f, true, sp, 2);
+    test_quad(1, 1, 2, 9, 9, 1, true, 5, 0.6f, 10.f, true, sp, 1);
+    test_quad(1, 1, 4, 2, 9, 0, true, 5, 0.6f, 10.f, true, sp, 1);
+    test_quad(1, 1, 3, 3, 3, 2, true, 5, 0.3f, 10.f, true, sp, 1);
   }
 }
 
@@ -1403,6 +1555,8 @@ static void fuzz(int rounds) {
   auto opick = [&](int lo, int hi) { return lo + (int)(go() % (unsigned)(hi - lo + 1)); };
   std::mt19937 gn(20261018);  // and the non-maximum-suppression cases from theirs
   auto npick = [&](int lo, int hi) { return lo + (int)(gn() % (unsigned)(hi - lo + 1)); };
+  std::mt19937 gq(20261019);  // and the sub-pixel refinement cases from theirs
+  auto qpick = [&](int lo, int hi) { return lo + (int)(gq() % (unsigned)(hi - lo + 1)); };
   for (int r = 0; r < rounds; ++r) {
     if (r % 10 == 9) {  // ScalePyramid octave: any chain, both stage-0 modes, sides from the largest tap count up, any grid
       const int which = opick(0, 4), planes = opick(1, 2), sp = opick(0, 2);
@@ -1430,6 +1584,12 @@ static void fuzz(int rounds) {
         case 8: test_nms3d<NMS3_MAX_VALUES>(1, npick(1, 2), npick(1, 5), H / 2 + 1, W, sp, grid); break;
         default: test_nms3d<NMS3_MINMAX>(npick(1, 2), npick(1, 2), npick(1, 6), H / 2 + 1, W, sp, grid); break;
       }
+    }
+    if (r % 10 == 7) {  // sub-pixel refinement: either form, with or without a mask, any parameters, shape and grid
+      const int n_iters = qpick(0, 6), radius = qpick(0, 2), mask = qpick(0, 1), allow = qpick(0, 1), sp = qpick(0, 1);
+      const float shift = qpick(0, 1) ? 0.6f : 0.3f, bonus = qpick(0, 1) ? 10.f : 0.f;
+      test_quad(qpick(1, 2), qpick(1, 2), qpick(1, 6), qpick(1, 24), qpick(1, 140), radius, mask, n_iters, shift, bonus, allow, sp,
+                (unsigned)qpick(1, 9));
     }
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
@@ -1547,6 +1707,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--nms") {
     test_nms_all();
     printf("%s: %d failing comparisons (non-maximum suppression, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--quad") {
+    test_quad_all();
+    printf("%s: %d failing comparisons (sub-pixel refinement, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {

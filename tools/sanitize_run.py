@@ -93,5 +93,11 @@ octv = torch.rand(1, 5, 2, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4)
 KG.nms3d(octv, (3, 3, 3), True)
 KG.nms3d(octv, (3, 3, 3))
 KG.nms3d_minmax(octv)
+# sub-pixel refinement on rough permuted (B, C, L, H, W) views with an odd width and partial tiles, so keypoints walk and
+# read patches across tiles: the conv form with nms3d_minmax's mask (C = 1, as the conv form must view its input) and the
+# iterative form computing its own NMS
+rough = torch.randn(1, 5, 1, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4)
+KG.conv_quad_interp3d(rough, 5, 10.0, 0.3, KG.nms3d_minmax(rough)[0], 2)
+KG.iterative_quad_interp3d(torch.randn(1, 5, 2, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4), 5, 10.0, 0.3)
 torch.cuda.synchronize()
 print("sanitize workload done")
