@@ -302,6 +302,23 @@ int kb200_quad_interp3d_forward(const void* x, const void* mask, void* coords, v
                                 int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Per-patch gradient histograms (feature/siftdesc.py SIFTDescriptor, feature/orientation.py
+ * PatchDominantGradientOrientation) in ONE kernel per call: each patch is read once and D or 1 floats are written, instead
+ * of about 100 (SIFT) or 290 (orientation) ATen kernels over the whole patch stack.
+ *   x        fp32 (N, 1, P, P) patches with column stride 1; sB, sH are the batch and row element strides
+ *   gk       contiguous fp32 P x P weighting (SIFT: the module's gk; orientation: its weighting)
+ *   pk       contiguous fp32 K x K pooling weights (pk.weight); smooth: the 5 taps of angular_smooth.weight
+ *   out      contiguous fp32 (N, A * S * S) descriptors or (N,) angles
+ * Envelope: P <= 64, ksize <= 64 and A * S * S <= 1024 (SIFT), P <= 64 and 2 <= A <= 64 (orientation); KB200_EUNSUPPORTED outside it.
+ * Each patch's result depends on that patch only (fixed-order sums, no atomics).  N = 0 launches nothing.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_sift_describe_forward(const void* x, const void* gk, const void* pk, void* out, long long N, int P, long long sB, long long sH,
+                                int num_ang_bins, int num_spatial_bins, int ksize, int stride, int pad, int rootsift, float clipval,
+                                float eps, int dtype, void* stream);
+int kb200_patch_orientation_forward(const void* x, const void* weighting, const void* smooth, void* out, long long N, int P, long long sB,
+                                    long long sH, int num_ang_bins, float eps, int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

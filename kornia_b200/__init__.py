@@ -27,9 +27,11 @@ def install(kornia_module=None) -> None:
     ``NonMaximaSuppression3d`` of the detectors and the sub-pixel refiners, and those refiners ``conv_quad_interp3d`` /
     ``iterative_quad_interp3d`` / ``ConvQuadInterp3d`` / ``IterativeQuadInterp3d`` / ``AdaptiveQuadInterp3d``) on an
     imported ``kornia`` package.  A defining module the package lacks, or a name its module does not define, is skipped.
-    Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``, ``MultiResolutionDetector`` or
-    ``SIFTFeatureScaleSpace`` built before ``install()`` keeps the reference pyramid, the reference
-    ``NonMaximaSuppression2d`` and the reference sub-pixel refiner it holds.
+    The per-keypoint stages of the SIFT-style pipelines are rebound too: ``SIFTDescriptor`` / ``sift_describe`` and
+    ``PatchDominantGradientOrientation``, which ``SIFTFeature``, ``SIFTFeatureScaleSpace`` and the ``LAFOrienter``
+    constructor build by name.  Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``,
+    ``MultiResolutionDetector``, ``SIFTFeature``, ``SIFTFeatureScaleSpace`` or ``LAFOrienter`` built before ``install()``
+    keeps the reference pyramid, ``NonMaximaSuppression2d``, sub-pixel refiner, descriptor and orienter it holds.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -78,6 +80,11 @@ def install(kornia_module=None) -> None:
         "ConvQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.ConvQuadInterp3d),
         "IterativeQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.IterativeQuadInterp3d),
         "AdaptiveQuadInterp3d": ("geometry.subpix.spatial_soft_argmax", geometry.subpix.AdaptiveQuadInterp3d),
+        # SIFTFeature / SIFTFeatureScaleSpace (integrated.py) build LAFDescriptor(SIFTDescriptor(41)) and the LAFOrienter
+        # constructor its PatchDominantGradientOrientation from these names
+        "SIFTDescriptor": ("feature.siftdesc", feature.SIFTDescriptor),
+        "sift_describe": ("feature.siftdesc", feature.sift_describe),
+        "PatchDominantGradientOrientation": ("feature.orientation", feature.PatchDominantGradientOrientation),
     }
     originals = {}
     for name, (mod, fn) in defining.items():

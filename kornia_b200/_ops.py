@@ -869,6 +869,88 @@ _define("quad_interp3d_fwd",
         lambda x, mask, *_: (x.new_empty((x.shape[0], x.shape[1], 3) + tuple(x.shape[2:])), torch.empty_like(x)))
 
 
+def _patches(x: torch.Tensor) -> torch.Tensor:
+    """``x`` (N, 1, P, P) itself when its column stride is 1 (the kernels take the batch and row strides), else a copy."""
+    return x if x.shape[-1] == 1 or x.stride(-1) == 1 else x.contiguous()
+
+
+def _check_patch_args(x: torch.Tensor, weighting: torch.Tensor, what: str) -> None:
+    """What the per-patch kernels read: (N, 1, P, P) patches and a P x P weighting of the patches' dtype and device."""
+    if x.dim() != 4 or x.shape[1] != 1 or x.shape[2] != x.shape[3]:
+        raise RuntimeError(f"kornia_b200: expected (N, 1, P, P) patches, got {tuple(x.shape)}")
+    P = x.shape[-1]
+    if weighting.numel() != P * P or weighting.shape[-2:] != (P, P):
+        raise RuntimeError(f"kornia_b200: {what} must be {P} x {P} for {P} x {P} patches, got {tuple(weighting.shape)}")
+    _fake_same_device(x, weighting)
+    _same(x, weighting, what)
+
+
+def _check_sift_args(x, gk, pk, num_ang_bins, num_spatial_bins, stride, pad) -> None:
+    _check_patch_args(x, gk, "gk")
+    K = pk.shape[-1]
+    if pk.dim() < 2 or pk.shape[-2] != K or pk.numel() != K * K or K < 1:
+        raise RuntimeError(f"kornia_b200: the pooling weights must be one square K x K kernel, got {tuple(pk.shape)}")
+    _fake_same_device(x, pk)
+    _same(x, pk, "the pooling weights")
+    if num_ang_bins < 1 or num_spatial_bins < 1 or stride < 1 or pad < 0:
+        raise RuntimeError(f"kornia_b200: bad SIFT configuration num_ang_bins={num_ang_bins} num_spatial_bins={num_spatial_bins} "
+                           f"stride={stride} pad={pad}")
+
+
+def _check_orientation_args(x, weighting, smooth, num_ang_bins) -> None:
+    _check_patch_args(x, weighting, "weighting")
+    if smooth.numel() != 5:
+        raise RuntimeError(f"kornia_b200: the angular smoothing must have 5 taps, got {tuple(smooth.shape)}")
+    _fake_same_device(x, smooth)
+    _same(x, smooth, "the angular smoothing")
+    if num_ang_bins < 1:
+        raise RuntimeError(f"kornia_b200: bad num_ang_bins={num_ang_bins}")
+
+
+def _sift_describe_cuda(x, gk, pk, num_ang_bins, num_spatial_bins, stride, pad, rootsift, clipval, eps):
+    """(N, A * S * S) descriptors of the (N, 1, P, P) patches ``x``; ``gk`` the P x P weighting, ``pk`` the K x K pooling weights."""
+    _require_cuda(x, "input")
+    _check_sift_args(x, gk, pk, num_ang_bins, num_spatial_bins, stride, pad)
+    N, P = x.shape[0], x.shape[-1]
+    out = torch.empty((N, num_ang_bins * num_spatial_bins ** 2), device=x.device, dtype=x.dtype)
+    if N == 0:
+        return out
+    xs, gkc, pkc = _patches(x), gk.contiguous(), pk.contiguous()
+    with torch.cuda.device(x.device), _Timed("sift_describe_forward", x):
+        _lib.call("kb200_sift_describe_forward", _ptr(xs), _ptr(gkc), _ptr(pkc), _ptr(out), N, P, xs.stride(0), xs.stride(-2), num_ang_bins,
+                  num_spatial_bins, pkc.shape[-1], stride, pad, int(rootsift), clipval, eps, _dtype_code(x), _stream(x))
+    _bump()
+    return out
+
+
+_define("sift_describe_fwd",
+        "(Tensor x, Tensor gk, Tensor pk, int num_ang_bins, int num_spatial_bins, int stride, int pad, bool rootsift, float clipval, "
+        "float eps) -> Tensor", _sift_describe_cuda,
+        lambda x, gk, pk, num_ang_bins, num_spatial_bins, stride, pad, *_: (_check_sift_args(x, gk, pk, num_ang_bins, num_spatial_bins, stride, pad),
+                                                                            x.new_empty((x.shape[0], num_ang_bins * num_spatial_bins ** 2)))[1])
+
+
+def _patch_orientation_cuda(x, weighting, smooth, num_ang_bins, eps):
+    """(N,) dominant gradient angles of the (N, 1, P, P) patches ``x``; ``smooth`` the 5 circular smoothing taps."""
+    _require_cuda(x, "input")
+    _check_orientation_args(x, weighting, smooth, num_ang_bins)
+    N, P = x.shape[0], x.shape[-1]
+    out = torch.empty((N,), device=x.device, dtype=x.dtype)
+    if N == 0:
+        return out
+    xs, wc, sc = _patches(x), weighting.contiguous(), smooth.contiguous()
+    with torch.cuda.device(x.device), _Timed("patch_orientation_forward", x):
+        _lib.call("kb200_patch_orientation_forward", _ptr(xs), _ptr(wc), _ptr(sc), _ptr(out), N, P, xs.stride(0), xs.stride(-2), num_ang_bins,
+                  eps, _dtype_code(x), _stream(x))
+    _bump()
+    return out
+
+
+_define("patch_orientation_fwd", "(Tensor x, Tensor weighting, Tensor smooth, int num_ang_bins, float eps) -> Tensor",
+        _patch_orientation_cuda,
+        lambda x, weighting, smooth, num_ang_bins, eps: (_check_orientation_args(x, weighting, smooth, num_ang_bins), x.new_empty((x.shape[0],)))[1])
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -1046,5 +1128,6 @@ OPERATORS: Tuple[str, ...] = (
     "warp_fwd", "warp_bwd", "warp_prelude", "warp_prelude_bwd", "remap_fwd", "remap_bwd", "filter2d_fwd", "filter2d_bwd_input",
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
-    "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd", "quad_interp3d_fwd",
+    "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd", "quad_interp3d_fwd", "sift_describe_fwd",
+    "patch_orientation_fwd",
 )

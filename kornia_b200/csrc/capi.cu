@@ -669,6 +669,48 @@ int kb200_quad_interp3d_forward(const void* x, const void* mask, void* coords, v
                                ysC, ysL, ysH, ysW, n_iters, radius, max_shift, bonus, add_bonus, allow_scale, (cudaStream_t)stream);
 }
 
+namespace kb200 {
+// siftdesc.cu / patch_orientation.cu (their kernels are not templates, so their headers are included there only)
+int sift_describe_forward(const float* x, const float* gk, const float* pk, float* out, long long N, int P, long long sB, long long sH, int A,
+                          int S, int K, int stride, int pad, int rootsift, float clipval, float eps, cudaStream_t st);
+int patch_orientation_forward(const float* x, const float* weighting, const float* smooth, float* out, long long N, int P, long long sB,
+                              long long sH, int A, float eps, cudaStream_t st);
+}  // namespace kb200
+
+int kb200_sift_describe_forward(const void* x, const void* gk, const void* pk, void* out, long long N, int P, long long sB, long long sH,
+                                int num_ang_bins, int num_spatial_bins, int ksize, int stride, int pad, int rootsift, float clipval,
+                                float eps, int dtype, void* stream) {
+  KB_CHECK_ARG(N >= 0 && P > 0 && num_ang_bins > 0 && num_spatial_bins > 0 && ksize > 0 && stride > 0 && pad >= 0,
+               "bad sizes N=%lld P=%d A=%d S=%d K=%d stride=%d pad=%d", N, P, num_ang_bins, num_spatial_bins, ksize, stride, pad);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused SIFT descriptor is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  if (N == 0) return KB200_OK;
+  KB_CHECK_ARG(x && gk && pk && out, "null pointer argument");
+  const int rc = sift_describe_forward((const float*)x, (const float*)gk, (const float*)pk, (float*)out, N, P, sB, sH, num_ang_bins,
+                                       num_spatial_bins, ksize, stride, pad, rootsift, clipval, eps, (cudaStream_t)stream);
+  if (rc == KB200_EUNSUPPORTED) set_error("SIFT configuration P=%d A=%d S=%d is outside the fused kernel's envelope", P, num_ang_bins, num_spatial_bins);
+  return rc;
+}
+
+int kb200_patch_orientation_forward(const void* x, const void* weighting, const void* smooth, void* out, long long N, int P, long long sB,
+                                    long long sH, int num_ang_bins, float eps, int dtype, void* stream) {
+  KB_CHECK_ARG(N >= 0 && P > 0 && num_ang_bins > 0, "bad sizes N=%lld P=%d A=%d", N, P, num_ang_bins);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused dominant-orientation estimate is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  if (N == 0) return KB200_OK;
+  KB_CHECK_ARG(x && weighting && smooth && out, "null pointer argument");
+  const int rc = patch_orientation_forward((const float*)x, (const float*)weighting, (const float*)smooth, (float*)out, N, P, sB, sH,
+                                           num_ang_bins, eps, (cudaStream_t)stream);
+  if (rc == KB200_EUNSUPPORTED) set_error("orientation configuration P=%d A=%d is outside the fused kernel's envelope", P, num_ang_bins);
+  return rc;
+}
+
 int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void* kernel_y, void* out, int B, int C, int H, int W,
                                  int Bkx, int kw, int Bky, int kh, int border, int same, double weight, int dtype, void* stream) {
   int rc = check_filter(x, kernel_x, B, C, H, W, Bkx, kh, kw, border, same, dtype);

@@ -3,6 +3,7 @@
 taps are bit-identical to the reference's and gradients w.r.t. ``sigma`` come from autograd."""
 from __future__ import annotations
 
+import math
 from typing import Optional, Union
 
 import torch
@@ -66,6 +67,75 @@ def get_gaussian_kernel2d(kernel_size, sigma, force_even: bool = False, *, devic
     col = get_gaussian_kernel1d(ky, sigma[:, 0, None], force_even, device=device, dtype=dtype)[..., None]
     row = get_gaussian_kernel1d(kx, sigma[:, 1, None], force_even, device=device, dtype=dtype)[..., None]
     return col * row.view(-1, 1, kx)
+
+
+# ---------------------------------------------------------------- discrete Gaussian (modified Bessel functions)
+# Polynomial approximations of I0 and I1 (Abramowitz & Stegun 9.8.1-9.8.4), for |x| < 3.75 in (x / 3.75)^2 and beyond
+# in 3.75 / |x|, highest power first.
+_I0_SMALL = (0.0045813, 0.0360768, 0.2659732, 1.2067492, 3.0899424, 3.5156229, 1.0)
+_I0_LARGE = (0.00392377, -0.01647633, 0.02635537, -0.02057706, 0.00916281, -0.00157565, 0.00225319, 0.01328592, 0.39894228)
+_I1_SMALL = (0.00032411, 0.00301532, 0.02658733, 0.15084934, 0.51498869, 0.87890594, 0.5)
+_I1_LARGE = (-0.00420059, 0.01787654, -0.02895312, 0.02282967, -0.01031555, 0.00163801, -0.00362018, -0.03988024, 0.39894228)
+
+
+def _horner(coeffs, y: torch.Tensor) -> torch.Tensor:
+    acc = torch.full_like(y, coeffs[0])
+    for c in coeffs[1:]:
+        acc = c + y * acc
+    return acc
+
+
+def _bessel_i0(x: torch.Tensor) -> torch.Tensor:
+    ax = x.abs()
+    small = _horner(_I0_SMALL, (x / 3.75) * (x / 3.75))
+    large = (ax.exp() / ax.sqrt()) * _horner(_I0_LARGE, 3.75 / ax)
+    return torch.where(ax < 3.75, small, large)
+
+
+def _bessel_i1(x: torch.Tensor) -> torch.Tensor:
+    ax = x.abs()
+    small = ax * _horner(_I1_SMALL, (x / 3.75) * (x / 3.75))
+    large = _horner(_I1_LARGE, 3.75 / ax) * ax.exp() / ax.sqrt()
+    return torch.where(ax < 3.75, small, torch.where(x < 0, -large, large))
+
+
+def _bessel_in(n: int, x: torch.Tensor) -> torch.Tensor:
+    """I_n(x), n >= 2, by Miller's downward recurrence I_{j-1} = I_{j+1} + (2 j / x) I_j normalised with I_0."""
+    zero = torch.isclose(x, torch.zeros((), device=x.device, dtype=x.dtype))
+    tox = 2.0 / torch.where(zero, torch.ones_like(x), x.abs())
+    ans, bip, bi = torch.zeros_like(x), torch.zeros_like(x), torch.ones_like(x)
+    for j in range(2 * (n + int(math.sqrt(40.0 * n))), 0, -1):
+        bip, bi = bi, bip + j * tox * bi
+        scale = torch.where(bi.abs() > 1.0e10, 1e-10, 1.0).to(x.dtype)
+        ans, bi, bip = ans * scale, bi * scale, bip * scale
+        if j == n:
+            ans = bip
+    out = ans * _bessel_i0(x) / bi
+    if n % 2 == 1:
+        out = torch.where(x < 0.0, -out, out)
+    return torch.where(zero, torch.zeros_like(x), out)
+
+
+def gaussian_discrete(window_size: int, sigma, *, device=None, dtype=None) -> torch.Tensor:
+    """(B, window_size) discrete Gaussian T(n, t) = exp(-t) I_n(t), t = sigma^2, for n = -(window_size // 2) ...
+    window_size // 2, each row normalised to sum 1.  ``sigma`` is a float or a (B, 1) tensor."""
+    if isinstance(sigma, float):
+        sigma = torch.tensor([[sigma]], device=device, dtype=dtype)
+    check_is_tensor(sigma)
+    check_shape(sigma, ["B", "1"])
+    t = sigma * sigma
+    half = int(window_size // 2)
+    orders = [_bessel_i0(t), _bessel_i1(t)] + [_bessel_in(n, t) for n in range(2, half + 1)]
+    out = torch.cat(orders[:0:-1] + orders, -1) * t.exp()
+    return out / out.sum(-1, keepdim=True)
+
+
+def get_gaussian_discrete_kernel1d(kernel_size: int, sigma: Union[float, torch.Tensor], force_even: bool = False, *,
+                                   device: Optional[torch.device] = None, dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """(B, kernel_size) discrete Gaussian taps (modified Bessel functions) with the reference's name and validation; the
+    angular smoothing of ``PatchDominantGradientOrientation`` is ``get_gaussian_discrete_kernel1d(5, 1.6)``."""
+    _check_kernel_size(kernel_size, allow_even=force_even)
+    return gaussian_discrete(kernel_size, sigma, device=device, dtype=dtype)
 
 
 # ---------------------------------------------------------------- box / laplacian / derivative taps

@@ -53,6 +53,7 @@ inline float __fsub_rn(float a, float b) { return a - b; }
 inline float __fdiv_rn(float a, float b) { return a / b; }
 inline float __fsqrt_rn(float a) { return sqrtf(a); }
 inline double __fma_rn(double a, double b, double c) { return fma(a, b, c); }
+inline float __double2float_rn(double a) { return (float)a; }
 inline double __dadd_rn(double a, double b) { return a + b; }
 inline double __dsub_rn(double a, double b) { return a - b; }
 inline double __dmul_rn(double a, double b) { return a * b; }

@@ -18,6 +18,8 @@
 #include "../../kornia_b200/csrc/octave_vwalk.cuh"
 #include "../../kornia_b200/csrc/nms.cuh"
 #include "../../kornia_b200/csrc/quad_interp.cuh"
+#include "../../kornia_b200/csrc/siftdesc.cuh"
+#include "../../kornia_b200/csrc/patch_orientation.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -40,6 +42,8 @@ alignas(128) unsigned char remap_smem[256 * 1024];
 alignas(128) unsigned char tma_smem[256 * 1024];
 alignas(128) unsigned char bwd2_smem[256 * 1024];
 alignas(128) unsigned char u8t_smem[256 * 1024];
+alignas(128) unsigned char sift_smem[128 * 1024];
+alignas(128) unsigned char ori_smem[128 * 1024];
 void set_error(const char*, ...) {}
 }  // namespace kb200
 
@@ -823,6 +827,221 @@ static void test_quad_all() {
   }
 }
 
+// ------------------------------------------------------------------------------------------ per-patch gradient histograms
+// Scalar restatement of SIFTDescriptor.forward / PatchDominantGradientOrientation.forward (kornia/feature/siftdesc.py,
+// orientation.py) in the kernels' summation order: the 3 x 3 gradient as every tap FMA'd from 0 in row-major order over a
+// replicate border, the reference's fp32 per-pixel ops one rounding each, (b0 == i) * w0 + (b1 == i) * w1 per bin, the
+// pooled cells and the histogram bins summed in fp64 in the kernels' order (a cell's window row-major; a bin's pixels lane by
+// lane, then the xor butterfly), the block sums per thread then per warp in order.  NaN matches NaN.
+static void ph_pixels(const float* patch, int P, const float (*st)[3][3], float eps, const float* weight, int A, bool add_pi,
+                      std::vector<int>& b0, std::vector<float>& w0, std::vector<float>& w1) {
+  const float pi = 3.14159274101257324219f, two_pi = 6.28318548202514648438f;
+  b0.assign(P * P, -1);
+  w0.assign(P * P, 0.f);
+  w1.assign(P * P, 0.f);
+  for (int y = 0; y < P; ++y)
+    for (int x = 0; x < P; ++x) {
+      float g[2] = {0.f, 0.f};
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) {
+          const float v = patch[std::min(std::max(y + r - 1, 0), P - 1) * P + std::min(std::max(x + c - 1, 0), P - 1)];
+          for (int o = 0; o < 2; ++o) g[o] = fmaf(st[o][r][c], v, g[o]);
+        }
+      const float gx2 = g[0] * g[0], gy2 = g[1] * g[1];
+      const float mag = sqrtf((gx2 + gy2) + eps) * weight[y * P + x];
+      const float ori = atan2f(g[1], g[0] + eps) + two_pi;
+      const float t = (float)A * (add_pi ? ori + pi : ori);
+      const float o_big = t / two_pi;
+      const float f = floorf(o_big), frac = o_big - f;
+      const int e = y * P + x;
+      if (!(f != f)) b0[e] = (((int)f % A) + A) % A;
+      w0[e] = (1.f - frac) * mag;
+      w1[e] = frac * mag;
+    }
+}
+static float ph_value(int b0, float w0, float w1, int i, int A) {
+  const int b1 = b0 < 0 ? -1 : (b0 + 1) % A;
+  const float a = (b0 == i ? 1.f : 0.f) * w0, b = (b1 == i ? 1.f : 0.f) * w1;
+  return a + b;
+}
+static double butterfly(double* v) {  // the xor butterfly of 32 lanes; every lane ends with lane 0's value
+  for (int o = 16; o > 0; o >>= 1) {
+    double nv[32];
+    for (int l = 0; l < 32; ++l) nv[l] = v[l] + v[l ^ o];
+    memcpy(v, nv, sizeof nv);
+  }
+  return v[0];
+}
+static double block_sum(const std::vector<double>& part) {  // PH_NT partials
+  double s = 0.0;
+  for (int w = 0; w < PH_NW; ++w) {
+    double lanes[32];
+    for (int l = 0; l < 32; ++l) lanes[l] = part[w * 32 + l];
+    const double ws = butterfly(lanes);
+    s = w == 0 ? ws : s + ws;
+  }
+  return s;
+}
+static float divisor(float n) { return n < 1e-12f ? 1e-12f : n; }
+
+static std::vector<float> make_patches(long long N, int P, long long sB, int sH, int specials) {
+  std::vector<float> x = randv((size_t)(N * sB));
+  if (specials) {
+    const float v[5] = {NAN, INFINITY, -INFINITY, -0.f, 1e-40f};
+    for (long long n = 1; n < N; n += 3) x[(size_t)(n * sB + (rng() % P) * sH + rng() % P)] = v[rng() % 5];
+  }
+  return x;
+}
+
+static void test_sift(long long N, int P, int A, int S, bool rootsift, float clipval, int specials, unsigned grid) {
+  const int K = 2 * (int)(P / (S + 1)), stride = P / S, pad = K / 4, D = A * S * S;
+  const int sH = P + 3;
+  const long long sB = (long long)sH * P + 5;
+  std::vector<float> x = make_patches(N, P, sB, sH, specials), gk = randv(P * P, 0.1f, 1.f), pk = randv(K * K, 0.1f, 1.f);
+  std::vector<float> got((size_t)(N * D), -777.f), want((size_t)(N * D));
+  SiftParams p{};
+  p.src = x.data();
+  p.gk = gk.data();
+  p.pk = pk.data();
+  p.out = got.data();
+  p.sB = sB;
+  p.sH = sH;
+  p.N = N;
+  p.P = P;
+  p.A = A;
+  p.S = S;
+  p.K = K;
+  p.stride = stride;
+  p.pad = pad;
+  p.rootsift = rootsift;
+  p.clipval = clipval;
+  p.eps = 1e-10f;
+  emu::launch(grid, dim3(PH_NT), [&] { sift_describe_kernel(p); });
+  const GradStencil st = diff_stencil();
+  std::vector<float> patch(P * P), desc(D);
+  std::vector<int> b0;
+  std::vector<float> w0, w1;
+  for (long long n = 0; n < N; ++n) {
+    for (int y = 0; y < P; ++y)
+      for (int xx = 0; xx < P; ++xx) patch[y * P + xx] = x[(size_t)(n * sB + y * sH + xx)];
+    ph_pixels(patch.data(), P, st.t, 1e-10f, gk.data(), A, false, b0, w0, w1);
+    std::vector<double> part(PH_NT, 0.0);
+    for (int c = 0; c < D; ++c) {
+      const int i = c / (S * S), cell = c % (S * S), y0 = (cell / S) * stride - pad, x0 = (cell % S) * stride - pad;
+      double acc = 0.0;
+      for (int ky = 0; ky < K; ++ky)
+        for (int kx = 0; kx < K; ++kx) {
+          const int y = y0 + ky, xx = x0 + kx;
+          const float v = (y >= 0 && y < P && xx >= 0 && xx < P) ? ph_value(b0[y * P + xx], w0[y * P + xx], w1[y * P + xx], i, A) : 0.f;
+          acc = fma((double)pk[ky * K + kx], (double)v, acc);
+        }
+      desc[c] = (float)acc;
+      part[c % PH_NT] = fma((double)desc[c], (double)desc[c], part[c % PH_NT]);
+    }
+    float div = divisor((float)sqrt(block_sum(part)));
+    std::fill(part.begin(), part.end(), 0.0);
+    for (int c = 0; c < D; ++c) {
+      float v = desc[c] / div;
+      if (v == v) v = std::min(std::max(v, 0.f), clipval);
+      desc[c] = v;
+      part[c % PH_NT] = fma((double)v, (double)v, part[c % PH_NT]);
+    }
+    div = divisor((float)sqrt(block_sum(part)));
+    float* out = want.data() + n * D;
+    if (rootsift) {
+      std::fill(part.begin(), part.end(), 0.0);
+      for (int c = 0; c < D; ++c) {
+        desc[c] = desc[c] / div;
+        part[c % PH_NT] += fabs((double)desc[c]);
+      }
+      div = divisor((float)block_sum(part));
+      for (int c = 0; c < D; ++c) out[c] = sqrtf(desc[c] / div + 1e-10f);
+    } else {
+      for (int c = 0; c < D; ++c) out[c] = desc[c] / div;
+    }
+  }
+  const std::string what = "sift_describe_kernel N=" + std::to_string(N) + " P=" + std::to_string(P) + " A=" + std::to_string(A) + " S=" +
+                           std::to_string(S) + (rootsift ? " rootsift" : " l2") + " clip=" + std::to_string(clipval) +
+                           (specials ? " special texels" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what, got.data(), want.data(), got.size());
+}
+
+static void test_orient(long long N, int P, int A, int specials, unsigned grid) {
+  const int sH = P + 1;
+  const long long sB = (long long)sH * P + 3;
+  std::vector<float> x = make_patches(N, P, sB, sH, specials), wt = randv(P * P, 0.1f, 1.f);
+  std::vector<float> smooth = {0.1f, 0.2f, 0.4f, 0.2f, 0.1f};
+  std::vector<float> got((size_t)N, -777.f), want((size_t)N);
+  OriParams p{};
+  p.src = x.data();
+  p.weighting = wt.data();
+  p.smooth = smooth.data();
+  p.out = got.data();
+  p.sB = sB;
+  p.sH = sH;
+  p.N = N;
+  p.P = P;
+  p.A = A;
+  p.eps = 1e-8f;
+  emu::launch(grid, dim3(PH_NT), [&] { patch_orientation_kernel(p); });
+  const GradStencil st = sobel_stencil();
+  const float pi = 3.14159274101257324219f, two_pi = 6.28318548202514648438f;
+  std::vector<float> patch(P * P), hist(A), sm(A);
+  std::vector<int> b0;
+  std::vector<float> w0, w1;
+  for (long long n = 0; n < N; ++n) {
+    for (int y = 0; y < P; ++y)
+      for (int xx = 0; xx < P; ++xx) patch[y * P + xx] = x[(size_t)(n * sB + y * sH + xx)];
+    ph_pixels(patch.data(), P, st.t, 1e-8f, wt.data(), A, true, b0, w0, w1);
+    for (int i = 0; i < A; ++i) {
+      double lanes[32];
+      for (int l = 0; l < 32; ++l) {
+        lanes[l] = 0.0;
+        for (int e = l; e < P * P; e += 32) lanes[l] += (double)ph_value(b0[e], w0[e], w1[e], i, A);
+      }
+      hist[i] = (float)(butterfly(lanes) / (double)(P * P));
+    }
+    for (int i = 0; i < A; ++i) {
+      float acc = 0.f;
+      for (int k = 0; k < 5; ++k) acc = fmaf(smooth[k], hist[((i + k - 2) % A + A) % A], acc);
+      sm[i] = acc;
+    }
+    int idx = 0;
+    for (int i = 1; i < A && sm[idx] == sm[idx]; ++i)
+      if (sm[i] > sm[idx] || sm[i] != sm[i]) idx = i;
+    const float c = sm[idx], l = sm[(A + idx - 1) % A], r = sm[(idx + 1) % A];
+    const float lr = l - r, half = 0.5f * lr, sum = l + r, c2 = 2.f * c, den = sum - c2, cs = half / den;
+    const float t = two_pi * ((float)idx + cs), q = t / (float)A;
+    want[n] = -(q - pi);
+  }
+  const std::string what = "patch_orientation_kernel N=" + std::to_string(N) + " P=" + std::to_string(P) + " A=" + std::to_string(A) +
+                           (specials ? " special texels" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what, got.data(), want.data(), got.size());
+}
+
+// The fixed lists (run_emu --sift / --orient): every configuration of the reference's tests and the envelope's edges, odd
+// batch sizes, grids that do not divide N, batch and row strides that are not P * P and P, special texels.
+static void test_sift_all() {
+  for (int sp = 0; sp < 2; ++sp) {
+    test_sift(7, 41, 8, 4, true, 0.2f, sp, 3);
+    test_sift(5, 32, 8, 4, false, 0.1f, sp, 2);
+    test_sift(3, 15, 8, 4, true, 0.2f, sp, 1);
+    test_sift(9, 19, 5, 3, true, 0.2f, sp, 4);
+    test_sift(4, 6, 4, 1, false, 0.2f, sp, 3);
+    test_sift(2, 64, 8, 4, true, 0.2f, sp, 1);
+    test_sift(3, 32, 16, 8, false, 0.2f, sp, 2);
+  }
+}
+static void test_orient_all() {
+  for (int sp = 0; sp < 2; ++sp) {
+    test_orient(11, 19, 36, sp, 4);
+    test_orient(5, 32, 36, sp, 2);
+    test_orient(7, 19, 8, sp, 3);
+    test_orient(3, 64, 64, sp, 2);
+    test_orient(6, 19, 2, sp, 5);
+  }
+}
+
 // ------------------------------------------------------------------------------------------ feature responses
 // Scalar restatement of kornia/feature/responses.py as this library composes it: spatial_gradient (replicate border,
 // row-major FMA over every tap), the products, gaussian_blur2d's row then column pass (reflect border, ascending FMA),
@@ -1557,6 +1776,7 @@ static void fuzz(int rounds) {
   auto npick = [&](int lo, int hi) { return lo + (int)(gn() % (unsigned)(hi - lo + 1)); };
   std::mt19937 gq(20261019);  // and the sub-pixel refinement cases from theirs
   auto qpick = [&](int lo, int hi) { return lo + (int)(gq() % (unsigned)(hi - lo + 1)); };
+  std::mt19937 gs(20261020);  // and the gradient-histogram cases from theirs
   for (int r = 0; r < rounds; ++r) {
     if (r % 10 == 9) {  // ScalePyramid octave: any chain, both stage-0 modes, sides from the largest tap count up, any grid
       const int which = opick(0, 4), planes = opick(1, 2), sp = opick(0, 2);
@@ -1590,6 +1810,13 @@ static void fuzz(int rounds) {
       const float shift = qpick(0, 1) ? 0.6f : 0.3f, bonus = qpick(0, 1) ? 10.f : 0.f;
       test_quad(qpick(1, 2), qpick(1, 2), qpick(1, 6), qpick(1, 24), qpick(1, 140), radius, mask, n_iters, shift, bonus, allow, sp,
                 (unsigned)qpick(1, 9));
+    }
+    if (r % 10 == 2) {  // per-patch gradient histograms: any envelope configuration, batch size and grid
+      auto spick = [&](int lo, int hi) { return lo + (int)(gs() % (unsigned)(hi - lo + 1)); };
+      static const int cfg[7][3] = {{41, 8, 4}, {32, 8, 4}, {15, 8, 4}, {19, 5, 3}, {6, 4, 1}, {64, 8, 4}, {32, 16, 8}};
+      const int* c = cfg[spick(0, 6)];
+      test_sift(spick(1, 9), c[0], c[1], c[2], c[0] != 6 && spick(0, 1), spick(0, 1) ? 0.2f : 0.1f, spick(0, 1), (unsigned)spick(1, 7));
+      test_orient(spick(1, 9), spick(0, 1) ? 19 : 32, spick(0, 1) ? 36 : spick(2, 64), spick(0, 1), (unsigned)spick(1, 7));
     }
     const int H = pick(1, 110), W = 4 * pick(1, 70), planes = pick(1, 4), lazy = pick(0, 1);
     const unsigned grid = (unsigned)pick(1, 9);
@@ -1712,6 +1939,15 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--quad") {
     test_quad_all();
     printf("%s: %d failing comparisons (sub-pixel refinement, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc >= 2 && (std::string(argv[1]) == "--sift" || std::string(argv[1]) == "--orient")) {
+    for (int a = 1; a < argc; ++a) {
+      if (std::string(argv[a]) == "--sift") test_sift_all();
+      if (std::string(argv[a]) == "--orient") test_orient_all();
+    }
+    printf("%s: %d failing comparisons (per-patch gradient histograms, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures,
+           emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {

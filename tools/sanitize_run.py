@@ -99,5 +99,10 @@ KG.nms3d_minmax(octv)
 rough = torch.randn(1, 5, 1, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4)
 KG.conv_quad_interp3d(rough, 5, 10.0, 0.3, KG.nms3d_minmax(rough)[0], 2)
 KG.iterative_quad_interp3d(torch.randn(1, 5, 2, 37, 61, generator=g).to(dev).permute(0, 2, 1, 3, 4), 5, 10.0, 0.3)
+# per-patch gradient histograms: SIFT on a batch-strided view of odd-sized patches (a grid that does not divide N) and the
+# dominant orientation at the reference's LAFOrienter size
+with torch.no_grad():
+    K.feature.SIFTDescriptor(19, 5, 3)(torch.rand(37, 1, 23, 23, generator=g).to(dev)[::2, :, 2:21, 1:20])
+    K.feature.PatchDominantGradientOrientation(19)(torch.rand(41, 1, 19, 19, generator=g).to(dev))
 torch.cuda.synchronize()
 print("sanitize workload done")
