@@ -2,9 +2,10 @@
 //
 // Replaces kornia/feature/responses.py:99-126 / :182-203: spatial_gradient (3x3 stencils, replicate border), dx^2, dy^2,
 // dx*dy, three gaussian_blur2d((7,7), (1,1)) calls (reflect border) and 7 (Harris) or ~17 (GFTT) elementwise kernels.
-// The skeleton is ssim_vwalk_kernel's: persistent CTAs walk 64-column bands top to bottom, the input box of each 32-row
-// tile arrives by TMA into a double-buffered slot, and the 6 row-filtered rows shared by vertically adjacent tiles are
-// carried in shared memory (three planes).  Arithmetic, one rounding per reference op, bit-identical to the composition:
+// The skeleton is ssim_vwalk_kernel's (vwalk.cuh): persistent CTAs walk 64-column bands top to bottom, the input box of
+// each 32-row tile arrives by TMA into a double-buffered slot, and the 6 row-filtered rows shared by vertically adjacent
+// tiles are carried in shared memory (three planes).  Arithmetic, one rounding per reference op, bit-identical to the
+// composition:
 //   * dx, dy with grad_tiled_kernel's tap order (row-major, ascending, every 3x3 tap including the zeros, __fmaf_rn);
 //   * the three products rounded once each; row sums with ascending FMA taps, column sums on column pairs (fma2_rn),
 //     as sepfilter_tiled_kernel;
@@ -17,9 +18,7 @@
 //
 // Launched by corner_vwalk.cu; tests/test_responses_gpu.py checks it bit for bit against the composition.
 #pragma once
-#include "sepfilter_tiled.cuh"
-#include "filter_generic.cuh"
-#include "ssim_vwalk.cuh"
+#include "vwalk.cuh"
 
 namespace kb200 {
 
@@ -38,7 +37,7 @@ struct CornerParams {
 };
 
 constexpr size_t corner_smem_bytes() {
-  return (size_t)(2 * (SSIMV_TH + 2) * SSIMV_BW + 3 * (SSIMV_TH + CORNER_K - 1) * SSIMV_TW) * sizeof(float) + 2 * sizeof(uint64_t);
+  return (size_t)(2 * (VWALK_TH + 2) * VWALK_BW + 3 * (VWALK_TH + CORNER_K - 1) * VWALK_TW) * sizeof(float) + 2 * sizeof(uint64_t);
 }
 
 // torch.minimum: NaN in either operand propagates (fminf would drop it)
@@ -60,20 +59,16 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
                                                               const __grid_constant__ CornerParams p) {
   static_assert(KIND == RESP_HARRIS || KIND == RESP_GFTT, "corner epilogues");
   constexpr int K = CORNER_K, HALO = K / 2, CARRY = K - 1;
-  constexpr int TW = SSIMV_TW, TH = SSIMV_TH, BW = SSIMV_BW;
+  constexpr int TW = VWALK_TW, TH = VWALK_TH, BW = VWALK_BW;
   constexpr int BH = TH + 2;                     // box rows: the tile's product rows and one stencil row on each side
   constexpr int MH = TH + CARRY;                 // rows of a row-filtered plane: image rows t*TH - HALO ... + MH
-  constexpr int COL0 = SSIMV_XPAD - HALO - 1;    // box column of the stencil window of product position 0
+  constexpr int COL0 = VWALK_XPAD - HALO - 1;    // box column of the stencil window of product position 0
   static_assert((COL0 & 3) == 0, "aligned stencil window");
   constexpr int WIN = 4 + K - 1;                 // product positions feeding 4 neighbouring outputs
   constexpr int NV = (WIN + 2 + 3) / 4;          // aligned float4 loads per stencil row
   constexpr int SLOT_FLOATS = BH * BW;
   constexpr uint32_t TILE_BYTES = BH * BW * 4, PRO_BYTES = (CARRY + 2) * BW * 4;
-  constexpr int QUADS = TW / 4;                  // 16 quads per row
-  constexpr int RPS = 256 / QUADS;               // 16 rows per sweep of the CTA
-  constexpr int SWEEPS = TH / RPS;               // 2
-  constexpr int RY = 4;                          // rows per thread in the column pass
-  static_assert((TW / 2) * (TH / RY) == 256 && SWEEPS * RPS == TH && CARRY <= RPS, "thread mapping");
+  constexpr int QUADS = VWALK_QUADS, RPS = VWALK_RPS, SWEEPS = VWALK_SWEEPS, RY = VWALK_RY;
   static_assert(COL0 + 4 * (QUADS - 1) + 4 * NV <= BW, "window loads stay inside a box row");
 
   extern __shared__ __align__(128) unsigned char corner_smem[];
@@ -82,53 +77,20 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
   uint64_t* full = reinterpret_cast<uint64_t*>(mid + 3 * MH * TW);  // [2]
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int bands = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * bands, tiles_y);
 
-  // box sequence of a band segment [t0, t1): prologue (t = t0 - 1), tile t0, ..., tile t1 - 1; issued two boxes ahead
-  struct Ahead {
-    int seg, strip, t0, t1, cursor, t, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {
-    if (ah.live && ah.t + 1 < ah.t1) {
-      ++ah.t;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.t0, ah.t1, ah.cursor);
-    ++ah.seg;
-    ah.t = ah.t0 - 1;
-    if (!first) ++ah.n;
+  // box sequence of a band segment [t0, t1): prologue (t = t0 - 1), tile t0, ..., tile t1 - 1
+  TileFeed<true> feed(segs);
+  auto load = [&](int slot, int strip, int t, bool prologue) {
+    const int plane = strip / bands, band = strip - plane * bands;
+    tma::mbar_arrive_expect_tx(&full[slot], prologue ? PRO_BYTES : TILE_BYTES);
+    tma::load_3d(slots + slot * SLOT_FLOATS, prologue ? &pro : &map, &full[slot], band * TW - VWALK_XPAD,
+                 prologue ? (t + 1) * TH - HALO - 1 : t * TH + HALO - 1, plane);  // the prologue: rows above tile t + 1
   };
-  auto issue = [&]() {
-    if (!ah.live) return;
-    const int plane = ah.strip / bands, band = ah.strip - plane * bands;
-    const int s = ah.n & 1;
-    float* slot = slots + s * SLOT_FLOATS;
-    tma::fence_proxy_async();
-    if (ah.t < ah.t0) {
-      tma::mbar_arrive_expect_tx(&full[s], PRO_BYTES);
-      tma::load_3d(slot, &pro, &full[s], band * TW - SSIMV_XPAD, ah.t0 * TH - HALO - 1, plane);
-    } else {
-      tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-      tma::load_3d(slot, &map, &full[s], band * TW - SSIMV_XPAD, ah.t * TH + HALO - 1, plane);
-    }
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   float g[K];
 #pragma unroll
@@ -142,7 +104,7 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
   int n = 0, strip, t0, t1, cursor = 0;
   for (int seg = 0; segs.get(seg, strip, t0, t1, cursor); ++seg) {
     const int plane = strip / bands, band = strip - plane * bands;
-    const int x0 = band * TW, ox = x0 - SSIMV_XPAD;
+    const int x0 = band * TW, ox = x0 - VWALK_XPAD;
     const size_t base = (size_t)plane * p.H * p.W;
     const float s4 = p.s4 ? __ldg(p.s4 + plane / p.C) : 1.0f;
     const int gq = x0 + 4 * rq;                                  // first output column of this thread's row-pass quad
@@ -156,16 +118,7 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
       const int oy = pro ? t0 * TH - HALO - 1 : t * TH + HALO - 1;  // image row of box row 0
       tma::mbar_wait(&full[s], (n >> 1) & 1);
 
-      if (ox < 0 || ox + BW > p.W || oy < 0 || oy + rows + 2 > p.H) {  // CTA-uniform: replicate border of the image
-        for (int e = tid; e < (rows + 2) * BW; e += 256) {
-          const int r = e / BW, c = e - r * BW;
-          const int gy = oy + r, gx = ox + c;
-          if ((unsigned)gy < (unsigned)p.H && (unsigned)gx < (unsigned)p.W) continue;
-          const int sr = border_index<KB200_REPLICATE>(gy, p.H) - oy, sc = border_index<KB200_REPLICATE>(gx, p.W) - ox;
-          if ((unsigned)sr < (unsigned)(rows + 2) && (unsigned)sc < (unsigned)BW) box[e] = box[sr * BW + sc];
-        }
-        __syncthreads();
-      }
+      patch_box_border<KB200_REPLICATE>(box, rows + 2, BW, ox, oy, p);  // replicate border of the image
 
       // ------------------------------------------------------------ row pass: dx, dy, products, three row sums
 #pragma unroll
@@ -227,42 +180,16 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
         }
       }
       __syncthreads();  // rows written, box consumed
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
       if (pro) continue;
 
       const int y0 = t * TH, gy0 = y0 - HALO;  // gy0: image row of mid row 0
-      if (gy0 < 0 || gy0 + MH > p.H) {         // CTA-uniform: first / last tiles of the band -- reflect row-filtered rows
-        for (int e = tid; e < MH * QUADS; e += 256) {
-          const int mr = e / QUADS, qd = e - mr * QUADS;
-          const int gy = gy0 + mr;
-          if ((unsigned)gy < (unsigned)p.H) continue;
-          const int sr = border_index<KB200_REFLECT>(gy, p.H) - gy0;  // an in-image row: never written by this loop
-          if ((unsigned)sr < (unsigned)MH) {
-#pragma unroll
-            for (int q = 0; q < 3; ++q) mid4[(q * MH + mr) * QUADS + qd] = mid4[(q * MH + sr) * QUADS + qd];
-          }
-        }
-        __syncthreads();
-      }
+      vwalk_reflect_rows<3, K>(mid4, gy0, p.H);  // first / last tiles of the band
 
       // ------------------------------------------------------------ column pass + response
       {
         float2 acc[3][RY];
-#pragma unroll
-        for (int q = 0; q < 3; ++q)
-#pragma unroll
-          for (int o = 0; o < RY; ++o) acc[q][o] = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < RY + K - 1; ++i) {
-#pragma unroll
-          for (int q = 0; q < 3; ++q) {
-            const float2 v = *reinterpret_cast<const float2*>(mid + (q * MH + rg * RY + i) * TW + 2 * cp);
-#pragma unroll
-            for (int o = 0; o < RY; ++o) {
-              if (i - o >= 0 && i - o < K) acc[q][o] = fma2_rn(make_float2(g[i - o], g[i - o]), v, acc[q][o]);
-            }
-          }
-        }
+        vwalk_column_pass<3, K>(mid, g, cp, rg, acc);
         const int gx = x0 + 2 * cp;
         if (gx < p.W) {  // W % 4 == 0: whole pairs
 #pragma unroll
@@ -281,18 +208,7 @@ __global__ void __launch_bounds__(256, 2) corner_vwalk_kernel(const __grid_const
         }
       }
       __syncthreads();  // every read of mid is done
-      if (t + 1 < t1) {
-        // carry rows [TH, MH) -> [0, CARRY) of the three planes: thread (rq, rr) moves exactly the cells it overwrites in
-        // the next row pass (mid row CARRY + rr + 16*it, quad rq)
-#pragma unroll
-        for (int it = 0; it < SWEEPS; ++it) {
-          const int R = CARRY + rr + it * RPS;
-          if (R >= TH) {
-#pragma unroll
-            for (int q = 0; q < 3; ++q) mid4[(q * MH + R - TH) * QUADS + rq] = mid4[(q * MH + R) * QUADS + rq];
-          }
-        }
-      }
+      if (t + 1 < t1) vwalk_carry_rows<3, K>(mid4, rq, rr);
     }
   }
 }

@@ -1,5 +1,6 @@
 // kornia_b200 -- host dispatch of the zero-skipping filter2d kernel (odd K from 9 to 31).
 #include "filter2d_taps.cuh"
+#include "persistent_launch.cuh"
 
 namespace kb200 {
 
@@ -16,16 +17,8 @@ static int launch_f2d_taps(const CUtensorMap& map, const F2dTapsParams& p, cudaS
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kern, 256, smem) != cudaSuccess || ctas < 1) ctas = 1;
     __atomic_store_n(&per_sm[p.K], ctas, __ATOMIC_RELAXED);
   }
-  const long long nstrips = (long long)p.planes * ceil_div(p.H, SEPT_TH);
-  const long long cap = (long long)ctas * sm_count();
-  const int grid = (int)(nstrips < cap ? nstrips : cap);
-  kern<<<grid, 256, smem, st>>>(map, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("filter2d_taps launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
+  kern<<<capped_grid((long long)p.planes * ceil_div(p.H, SEPT_TH), ctas), 256, smem, st>>>(map, p);
+  return launch_status("filter2d_taps");
 }
 
 int filter2d_taps_forward(const float* x, const float* k, float* out, int B, int C, int H, int W, int Bk, int kh, int kw, int border,
@@ -36,16 +29,8 @@ int filter2d_taps_forward(const float* x, const float* k, float* out, int B, int
   const int halo = (kw - 1) / 2;
   if (border != KB200_CONSTANT && (H <= halo || W <= halo)) return KB200_EUNSUPPORTED;
   if ((long long)B * C * ceil_div(H, SEPT_TH) > 0x7fffffffll) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
   CUtensorMap map;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * C};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)F2DT_BW, (cuuint32_t)(SEPT_TH + kw - 1), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  if (encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return KB200_EUNSUPPORTED;
+  if (!encode_plane_map(&map, x, (long long)B * C, H, W, F2DT_BW, SEPT_TH + kw - 1)) return KB200_EUNSUPPORTED;
   F2dTapsParams p{k, out, C, H, W, Bk, B * C, kw};
   if (border == KB200_CONSTANT) return launch_f2d_taps<KB200_CONSTANT>(map, p, st);
   if (border == KB200_REFLECT) return launch_f2d_taps<KB200_REFLECT>(map, p, st);

@@ -92,46 +92,18 @@ __global__ void __launch_bounds__(256, 2) filter2d_taps_kernel(const __grid_cons
   float* v_tiny = reinterpret_cast<float*>(n_taps + 1);
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int tiles_x = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * tiles_y, tiles_x);
 
-  struct Ahead {
-    int seg, strip, tx0, tx1, cursor, tx, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {
-    if (ah.live && ah.tx + 1 < ah.tx1) {
-      ++ah.tx;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.tx0, ah.tx1, ah.cursor);
-    ++ah.seg;
-    ah.tx = ah.tx0;
-    if (!first) ++ah.n;
+  TileFeed<false> feed(segs);
+  auto load = [&](int slot, int strip, int tx, bool) {
+    const int plane = strip / tiles_y, ty = strip - plane * tiles_y;
+    tma::mbar_arrive_expect_tx(&full[slot], TILE_BYTES);
+    tma::load_3d(tiles + slot * TILE_FLOATS, &tmap, &full[slot], tx * TW - F2DT_XPAD, ty * TH - HALO, plane);
   };
-  auto issue = [&]() {
-    if (!ah.live) return;
-    const int plane = ah.strip / tiles_y, ty = ah.strip - plane * tiles_y;
-    const int s = ah.n & 1;
-    tma::fence_proxy_async();
-    tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-    tma::load_3d(tiles + s * TILE_FLOATS, &tmap, &full[s], ah.tx * TW - F2DT_XPAD, ty * TH - HALO, plane);
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   const int q = tid & 31, rg = tid >> 5;  // columns q + 32 c, rows 4 rg + o of the tile
   const int col0 = F2DT_XPAD - HALO;      // box column of the first tap of output column 0
@@ -157,20 +129,7 @@ __global__ void __launch_bounds__(256, 2) filter2d_taps_kernel(const __grid_cons
       float* tile = tiles + s * TILE_FLOATS;
       tma::mbar_wait(&full[s], (n >> 1) & 1);
 
-      if (BORDER != KB200_CONSTANT) {
-        const int ox = tx * TW - F2DT_XPAD, oy = y0 - HALO;
-        if (ox < 0 || oy < 0 || ox + BW > p.W || oy + BH > p.H) {
-          for (int e = tid; e < TILE_FLOATS; e += 256) {
-            const int r = e / BW, c = e - r * BW;
-            const int gy = oy + r, gx = ox + c;
-            if ((unsigned)gy < (unsigned)p.H && (unsigned)gx < (unsigned)p.W) continue;
-            const int sr = border_index<BORDER>(gy, p.H) - oy, sc = border_index<BORDER>(gx, p.W) - ox;
-            // the folded source of every cell an output of this tile reads lies inside the box (H, W > halo)
-            if ((unsigned)sr < (unsigned)BH && (unsigned)sc < (unsigned)BW) tile[e] = tile[sr * BW + sc];
-          }
-          __syncthreads();
-        }
-      }
+      patch_box_border<BORDER>(tile, BH, BW, tx * TW - F2DT_XPAD, y0 - HALO, p);
 
       bool unsafe = false;
       {
@@ -210,7 +169,7 @@ __global__ void __launch_bounds__(256, 2) filter2d_taps_kernel(const __grid_cons
           }
       }
       __syncthreads();  // tile[s] consumed by every thread
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
 
       if (rows_full && (tx + 1) * TW <= p.W) {
 #pragma unroll

@@ -1,36 +1,17 @@
 // kornia_b200 -- host dispatch of the tiled small-kernel filter2d.
 #include "filter2d_tiled.cuh"
+#include "persistent_launch.cuh"
 
 namespace kb200 {
 
 template <int K, int BORDER, bool DOWN2 = false>
 static int launch_f2d_tiled(const CUtensorMap& map, const F2dTiledParams& p, cudaStream_t st) {
-  constexpr int BH = SEPT_TH + K - 1;
-  constexpr size_t smem = (size_t)(2 * BH * SEPT_BW) * 4 + 2 * sizeof(uint64_t);
+  constexpr size_t smem = f2d_tiled_smem_bytes<K>();
   auto kern = filter2d_tiled_kernel<K, BORDER, DOWN2>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   KB_SET_SMEM_ONCE(configured, kern, smem);
-  const long long nstrips = (long long)p.planes * ceil_div(p.H, SEPT_TH);
-  const long long cap = 3ll * sm_count();
-  const int grid = (int)(nstrips < cap ? nstrips : cap);
-  kern<<<grid, 256, smem, st>>>(map, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("filter2d_tiled launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
-}
-
-static bool encode_plane_map(CUtensorMap* map, const float* x, int planes, int H, int W, int box_h) {
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return false;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)planes};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)SEPT_BW, (cuuint32_t)box_h, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  kern<<<capped_grid((long long)p.planes * ceil_div(p.H, SEPT_TH), 3), 256, smem, st>>>(map, p);
+  return launch_status("filter2d_tiled");
 }
 
 // pyrdown in one pass (filter2d_tiled_kernel<5, BORDER, DOWN2 = true>).  KB200_EUNSUPPORTED -> the host composes
@@ -41,7 +22,7 @@ int pyrdown_tiled_forward(const float* x, const float* k, float* out, int B, int
   if (border != KB200_CONSTANT && (H <= 2 || W <= 2)) return KB200_EUNSUPPORTED;
   if ((long long)B * C * ceil_div(H, SEPT_TH) > 0x7fffffffll) return KB200_EUNSUPPORTED;
   CUtensorMap map;
-  if (!encode_plane_map(&map, x, B * C, H, W, SEPT_TH + 4)) return KB200_EUNSUPPORTED;
+  if (!encode_plane_map(&map, x, (long long)B * C, H, W, SEPT_BW, SEPT_TH + 4)) return KB200_EUNSUPPORTED;
   F2dTiledParams p{k, out, C, H, W, Bk, B * C};
   if (border == KB200_CONSTANT) return launch_f2d_tiled<5, KB200_CONSTANT, true>(map, p, st);
   if (border == KB200_REFLECT) return launch_f2d_tiled<5, KB200_REFLECT, true>(map, p, st);
@@ -57,16 +38,8 @@ int filter2d_tiled_forward(const float* x, const float* k, float* out, int B, in
   const int halo = (kw - 1) / 2;
   if (border != KB200_CONSTANT && (H <= halo || W <= halo)) return KB200_EUNSUPPORTED;
   if ((long long)B * C * ceil_div(H, SEPT_TH) > 0x7fffffffll) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
   CUtensorMap map;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * C};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)SEPT_BW, (cuuint32_t)(SEPT_TH + kw - 1), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  if (encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return KB200_EUNSUPPORTED;
+  if (!encode_plane_map(&map, x, (long long)B * C, H, W, SEPT_BW, SEPT_TH + kw - 1)) return KB200_EUNSUPPORTED;
   F2dTiledParams p{k, out, C, H, W, Bk, B * C};
 #define KB_F2D_CASE(K_)                                                                    \
   if (kw == K_) {                                                                          \

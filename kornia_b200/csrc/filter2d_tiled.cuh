@@ -25,6 +25,11 @@ struct F2dTiledParams {
   int C, H, W, Bk, planes;
 };
 
+template <int K>
+constexpr size_t f2d_tiled_smem_bytes() {  // two boxes, two mbarriers
+  return (size_t)(2 * (SEPT_TH + K - 1) * SEPT_BW) * 4 + 2 * sizeof(uint64_t);
+}
+
 template <int K, int BORDER, bool DOWN2 = false>
 __global__ void __launch_bounds__(256, 3) filter2d_tiled_kernel(const __grid_constant__ CUtensorMap tmap,
                                                                 const __grid_constant__ F2dTiledParams p) {
@@ -38,51 +43,23 @@ __global__ void __launch_bounds__(256, 3) filter2d_tiled_kernel(const __grid_con
   constexpr uint32_t TILE_BYTES = TILE_FLOATS * 4;
   static_assert(TW / 4 == 32 && TH / 4 == 8, "thread mapping: 32 quads x 8 row groups");
 
-  extern __shared__ __align__(128) unsigned char f2d_smem[];
+  extern __shared__ __align__(128) unsigned char f2d_smem[];  // f2d_tiled_smem_bytes<K>()
   float* tiles = reinterpret_cast<float*>(f2d_smem);  // [2][BH][BW]
   uint64_t* full = reinterpret_cast<uint64_t*>(tiles + 2 * TILE_FLOATS);
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int tiles_x = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * tiles_y, tiles_x);
 
-  struct Ahead {
-    int seg, strip, tx0, tx1, cursor, tx, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {
-    if (ah.live && ah.tx + 1 < ah.tx1) {
-      ++ah.tx;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.tx0, ah.tx1, ah.cursor);
-    ++ah.seg;
-    ah.tx = ah.tx0;
-    if (!first) ++ah.n;
+  TileFeed<false> feed(segs);
+  auto load = [&](int slot, int strip, int tx, bool) {
+    const int plane = strip / tiles_y, ty = strip - plane * tiles_y;
+    tma::mbar_arrive_expect_tx(&full[slot], TILE_BYTES);
+    tma::load_3d(tiles + slot * TILE_FLOATS, &tmap, &full[slot], tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
   };
-  auto issue = [&]() {
-    if (!ah.live) return;
-    const int plane = ah.strip / tiles_y, ty = ah.strip - plane * tiles_y;
-    const int s = ah.n & 1;
-    tma::fence_proxy_async();
-    tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-    tma::load_3d(tiles + s * TILE_FLOATS, &tmap, &full[s], ah.tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   const int q = tid & 31, rg = tid >> 5;  // quad q (columns 4q..4q+3) of rows 4*rg .. 4*rg+3
 
@@ -104,19 +81,7 @@ __global__ void __launch_bounds__(256, 3) filter2d_tiled_kernel(const __grid_con
       float* tile = tiles + s * TILE_FLOATS;
       tma::mbar_wait(&full[s], (n >> 1) & 1);
 
-      if (BORDER != KB200_CONSTANT) {
-        const int ox = tx * TW - SEPT_XPAD, oy = y0 - HALO;
-        if (ox < 0 || oy < 0 || ox + BW > p.W || oy + BH > p.H) {
-          for (int e = tid; e < BH * BW; e += 256) {
-            const int r = e / BW, c = e - r * BW;
-            const int gy = oy + r, gx = ox + c;
-            if ((unsigned)gy < (unsigned)p.H && (unsigned)gx < (unsigned)p.W) continue;
-            const int sr = border_index<BORDER>(gy, p.H) - oy, sc = border_index<BORDER>(gx, p.W) - ox;
-            if ((unsigned)sr < (unsigned)BH && (unsigned)sc < (unsigned)BW) tile[e] = tile[sr * BW + sc];
-          }
-          __syncthreads();
-        }
-      }
+      patch_box_border<BORDER>(tile, BH, BW, tx * TW - SEPT_XPAD, y0 - HALO, p);
 
       // 4 x 4 outputs per thread; rows enter the register window one at a time, each feeding up to K output rows
       float acc[4][4];
@@ -147,7 +112,7 @@ __global__ void __launch_bounds__(256, 3) filter2d_tiled_kernel(const __grid_con
         }
       }
       __syncthreads();  // tile[s] consumed by every thread
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
 
       if (DOWN2) {
         if (tx * TW + 4 * q < p.W) {

@@ -1,25 +1,17 @@
 // kornia_b200 -- host dispatch of the tiled image-derivative kernel (gradient_tiled.cuh).
 #include "gradient_tiled.cuh"
+#include "persistent_launch.cuh"
 
 namespace kb200 {
 
 template <int K, int NOUT, GradEpilogue E>
 static int launch_grad_tiled(const CUtensorMap& map, const GradTiledParams& p, cudaStream_t st) {
-  constexpr int BH = SEPT_TH + K - 1;
-  constexpr size_t smem = (size_t)(2 * BH * SEPT_BW) * 4 + 2 * sizeof(uint64_t);
+  constexpr size_t smem = grad_tiled_smem_bytes<K>();
   auto kern = grad_tiled_kernel<K, NOUT, E>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   KB_SET_SMEM_ONCE(configured, kern, smem);
-  const long long nstrips = (long long)p.planes * ceil_div(p.H, SEPT_TH);
-  const long long cap = (long long)grad_tiled_ctas<K, E>() * sm_count();
-  const int grid = (int)(nstrips < cap ? nstrips : cap);
-  kern<<<grid, 256, smem, st>>>(map, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("grad_tiled launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
+  kern<<<capped_grid((long long)p.planes * ceil_div(p.H, SEPT_TH), grad_tiled_ctas<K, E>()), 256, smem, st>>>(map, p);
+  return launch_status("grad_tiled");
 }
 
 // tensor map and parameters shared by every epilogue; false outside the kernel's envelope
@@ -28,15 +20,7 @@ static bool grad_tiled_setup(const float* x, const double* taps, float* out, int
   if ((W % 4) != 0 || (reinterpret_cast<uintptr_t>(x) & 15) != 0 || (reinterpret_cast<uintptr_t>(out) & 15) != 0) return false;
   if (H <= k / 2 || W <= k / 2) return false;
   if ((long long)planes * ceil_div(H, SEPT_TH) > 0x7fffffffll) return false;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return false;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)planes};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)SEPT_BW, (cuuint32_t)(SEPT_TH + k - 1), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  if (encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return false;
+  if (!encode_plane_map(&map, x, planes, H, W, SEPT_BW, SEPT_TH + k - 1)) return false;
   p.out = out;
   p.H = H;
   p.W = W;

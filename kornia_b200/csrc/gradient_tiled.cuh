@@ -34,6 +34,11 @@ constexpr int grad_tiled_ctas() {
   return E == GRAD_HESS && K == 5 ? 2 : 3;
 }
 
+template <int K>
+constexpr size_t grad_tiled_smem_bytes() {  // two boxes, two mbarriers
+  return (size_t)(2 * (SEPT_TH + K - 1) * SEPT_BW) * 4 + 2 * sizeof(uint64_t);
+}
+
 template <int K, int NOUT, GradEpilogue E>
 __global__ void __launch_bounds__(256, grad_tiled_ctas<K, E>()) grad_tiled_kernel(const __grid_constant__ CUtensorMap tmap,
                                                             const __grid_constant__ GradTiledParams p) {
@@ -51,51 +56,23 @@ __global__ void __launch_bounds__(256, grad_tiled_ctas<K, E>()) grad_tiled_kerne
   constexpr int SWEEPS = TH / (8 * R);      // 8 row groups of R rows per sweep
   static_assert(TW / 4 == 32 && SWEEPS * 8 * R == TH, "thread mapping: 32 quads x 8 row groups x SWEEPS");
 
-  extern __shared__ __align__(128) unsigned char gradt_smem[];
+  extern __shared__ __align__(128) unsigned char gradt_smem[];  // grad_tiled_smem_bytes<K>()
   float* tiles = reinterpret_cast<float*>(gradt_smem);  // [2][BH][BW]
   uint64_t* full = reinterpret_cast<uint64_t*>(tiles + 2 * TILE_FLOATS);
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int tiles_x = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * tiles_y, tiles_x);
 
-  struct Ahead {
-    int seg, strip, tx0, tx1, cursor, tx, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {
-    if (ah.live && ah.tx + 1 < ah.tx1) {
-      ++ah.tx;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.tx0, ah.tx1, ah.cursor);
-    ++ah.seg;
-    ah.tx = ah.tx0;
-    if (!first) ++ah.n;
+  TileFeed<false> feed(segs);
+  auto load = [&](int slot, int strip, int tx, bool) {
+    const int plane = strip / tiles_y, ty = strip - plane * tiles_y;
+    tma::mbar_arrive_expect_tx(&full[slot], TILE_BYTES);
+    tma::load_3d(tiles + slot * TILE_FLOATS, &tmap, &full[slot], tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
   };
-  auto issue = [&]() {
-    if (!ah.live) return;
-    const int plane = ah.strip / tiles_y, ty = ah.strip - plane * tiles_y;
-    const int s = ah.n & 1;
-    tma::fence_proxy_async();
-    tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-    tma::load_3d(tiles + s * TILE_FLOATS, &tmap, &full[s], ah.tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   const int q = tid & 31, rg = tid >> 5;  // quad q (columns 4q..4q+3), row group rg
   const size_t HW = (size_t)p.H * p.W;
@@ -112,19 +89,8 @@ __global__ void __launch_bounds__(256, grad_tiled_ctas<K, E>()) grad_tiled_kerne
       float* tile = tiles + s * TILE_FLOATS;
       tma::mbar_wait(&full[s], (n >> 1) & 1);
 
-      {  // replicate border: cells of the box outside the image copy the nearest image cell (which lies inside the box)
-        const int ox = tx * TW - SEPT_XPAD, oy = y0 - HALO;
-        if (ox < 0 || oy < 0 || ox + BW > p.W || oy + BH > p.H) {
-          for (int e = tid; e < BH * BW; e += 256) {
-            const int r = e / BW, c = e - r * BW;
-            const int gy = oy + r, gx = ox + c;
-            if ((unsigned)gy < (unsigned)p.H && (unsigned)gx < (unsigned)p.W) continue;
-            const int sr = border_index<KB200_REPLICATE>(gy, p.H) - oy, sc = border_index<KB200_REPLICATE>(gx, p.W) - ox;
-            if ((unsigned)sr < (unsigned)BH && (unsigned)sc < (unsigned)BW) tile[e] = tile[sr * BW + sc];
-          }
-          __syncthreads();
-        }
-      }
+      // replicate border: cells of the box outside the image copy the nearest image cell (which lies inside the box)
+      patch_box_border<KB200_REPLICATE>(tile, BH, BW, tx * TW - SEPT_XPAD, y0 - HALO, p);
 
       const int gx0 = tx * TW + 4 * q;
 #pragma unroll
@@ -192,7 +158,7 @@ __global__ void __launch_bounds__(256, grad_tiled_ctas<K, E>()) grad_tiled_kerne
         }
       }
       __syncthreads();  // tile[s] consumed by every thread
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
     }
   }
 }

@@ -1,5 +1,6 @@
 // kornia_b200 -- host side of the ScalePyramid octave kernel (octave_vwalk.cuh).
 #include "octave_vwalk.cuh"
+#include "persistent_launch.cuh"
 
 namespace kb200 {
 
@@ -12,15 +13,8 @@ static int launch_octave(const OctaveParams& p, cudaStream_t st) {
   const long long steps = ceil_div(p.H + CH::D(CH::L - 1), OCT_TH);
   // segments of at least 3 PRIME steps, so a segment that starts inside a band spends at most a quarter of its steps refilling
   const long long want = strips * steps / (3 * CH::PRIME() > 0 ? 3 * CH::PRIME() : 1);
-  const long long cap = sm_count();
-  const int grid = (int)(want < 1 ? 1 : want < cap ? want : cap);
-  kern<<<grid, OCT_NT, CH::SMEM_BYTES(), st>>>(p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("octave_vwalk launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
+  kern<<<capped_grid(want < 1 ? 1 : want, 1), OCT_NT, CH::SMEM_BYTES(), st>>>(p);
+  return launch_status("octave_vwalk");
 }
 
 template <typename CH>

@@ -27,7 +27,7 @@
 // tools/hostemu (run_emu --octave) runs it on the host.
 #pragma once
 #include "filter_generic.cuh"
-#include "warp_tma.cuh"
+#include "tma.cuh"
 
 namespace kb200 {
 

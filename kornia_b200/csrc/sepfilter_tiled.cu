@@ -1,25 +1,17 @@
 // kornia_b200 -- host dispatch of the tiled separable filter.
+#include "persistent_launch.cuh"
 #include "sepfilter_tiled.cuh"
 
 namespace kb200 {
 
 template <int K, int BORDER, bool LERP = false>
 static int launch_sep_tiled(const CUtensorMap& map, const SepTiledParams& p, cudaStream_t st) {
-  constexpr int BH = SEPT_TH + K - 1;
-  constexpr size_t smem = (size_t)(2 * BH * SEPT_BW + BH * SEPT_TW) * 4 + 2 * sizeof(uint64_t);
+  constexpr size_t smem = sept_smem_bytes<K>();
   auto kern = sepfilter_tiled_kernel<K, BORDER, LERP>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   KB_SET_SMEM_ONCE(configured, kern, smem);
-  const long long nstrips = (long long)p.planes * ceil_div(p.H, SEPT_TH);
-  const long long cap = 3ll * sm_count();
-  const int grid = (int)(nstrips < cap ? nstrips : cap);
-  kern<<<grid, 256, smem, st>>>(map, p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("sepfilter_tiled launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
+  kern<<<capped_grid((long long)p.planes * ceil_div(p.H, SEPT_TH), 3), 256, smem, st>>>(map, p);
+  return launch_status("sepfilter_tiled");
 }
 
 // KB200_EUNSUPPORTED -> caller uses sepfilter_fwd_generic (circular border, 'valid', even / non-square /
@@ -32,17 +24,8 @@ int sepfilter_tiled_forward(const float* x, const float* kx, const float* ky, fl
   const int halo = (kw - 1) / 2;
   if (border != KB200_CONSTANT && (H <= halo || W <= halo)) return KB200_EUNSUPPORTED;  // fold source must be in the box
   if ((long long)B * C * ceil_div(H, SEPT_TH) > 0x7fffffffll) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
   CUtensorMap map;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * C};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t box[3] = {(cuuint32_t)SEPT_BW, (cuuint32_t)(SEPT_TH + kw - 1), 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult cr = encode(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return KB200_EUNSUPPORTED;
+  if (!encode_plane_map(&map, x, (long long)B * C, H, W, SEPT_BW, SEPT_TH + kw - 1)) return KB200_EUNSUPPORTED;
   SepTiledParams p{kx, ky, out, C, H, W, Bkx, Bky, B * C, x, lerp_w ? *lerp_w : 0.f};
   if (lerp_w) {
     if (kw > 11 || (reinterpret_cast<uintptr_t>(x) & 7) != 0) return KB200_EUNSUPPORTED;

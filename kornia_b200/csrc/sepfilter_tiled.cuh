@@ -19,11 +19,7 @@
 // element (two padded copies, two conv passes).  Tap order (ascending, FMA) is the generic kernel's,
 // so the two agree bit for bit.
 #pragma once
-#include <cuda.h>
-#include <cudaTypedefs.h>
-
-#include "filter_generic.cuh"
-#include "warp_tma.cuh"
+#include "tile_feed.cuh"
 
 namespace kb200 {
 
@@ -48,6 +44,11 @@ __device__ __forceinline__ float lerp_like_torch(float start, float end, float w
   return fabsf(w) < 0.5f ? fmaf(w, diff, start) : fmaf(-diff, __fsub_rn(1.f, w), end);
 }
 
+template <int K>
+constexpr size_t sept_smem_bytes() {  // two boxes, the row-filtered tile, two mbarriers
+  return (size_t)(2 * (SEPT_TH + K - 1) * SEPT_BW + (SEPT_TH + K - 1) * SEPT_TW) * 4 + 2 * sizeof(uint64_t);
+}
+
 // LERP: the epilogue blends the filtered value with the input, out = lerp(filtered, x, w) -- unsharp_mask
 // (filters/unsharp.py:53-54: gaussian_blur2d, then a separate torch.lerp pass over three full-size tensors) in the
 // blur's own pass.
@@ -68,53 +69,24 @@ __global__ void __launch_bounds__(256, 3) sepfilter_tiled_kernel(const __grid_co
   constexpr int RY = 8;
   static_assert((TW / 2) * (TH / RY) == 256 && TW / 4 == 32, "thread mapping");
 
-  extern __shared__ __align__(128) unsigned char sept_smem[];
+  extern __shared__ __align__(128) unsigned char sept_smem[];  // sept_smem_bytes<K>()
   float* tiles = reinterpret_cast<float*>(sept_smem);  // [2][BH][BW]
   float* mid = tiles + 2 * TILE_FLOATS;                // [BH][TW]
   uint64_t* full = reinterpret_cast<uint64_t*>(mid + BH * TW);  // [2]
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int tiles_x = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * tiles_y, tiles_x);
 
-  // The issuing thread walks the same tile sequence as the CTA, two tiles ahead.
-  struct Ahead {
-    int seg, strip, tx0, tx1, cursor, tx, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {  // advance to the next tile (or the first), called by one thread
-    if (ah.live && ah.tx + 1 < ah.tx1) {
-      ++ah.tx;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.tx0, ah.tx1, ah.cursor);
-    ++ah.seg;
-    ah.tx = ah.tx0;
-    if (!first) ++ah.n;
+  TileFeed<false> feed(segs);
+  auto load = [&](int slot, int strip, int tx, bool) {
+    const int plane = strip / tiles_y, ty = strip - plane * tiles_y;
+    tma::mbar_arrive_expect_tx(&full[slot], TILE_BYTES);
+    tma::load_3d(tiles + slot * TILE_FLOATS, &tmap, &full[slot], tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
   };
-  auto issue = [&]() {  // load the tile `ah` points at, then step
-    if (!ah.live) return;
-    const int plane = ah.strip / tiles_y, ty = ah.strip - plane * tiles_y;
-    const int s = ah.n & 1;
-    tma::fence_proxy_async();
-    tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-    tma::load_3d(tiles + s * TILE_FLOATS, &tmap, &full[s], ah.tx * TW - SEPT_XPAD, ty * TH - HALO, plane);
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();  // -> first tile
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   // thread roles (fixed for the whole kernel)
   const int rq = tid & 31, rr = tid >> 5;      // row pass: quad rq of rows rr, rr+8, ...
@@ -142,21 +114,7 @@ __global__ void __launch_bounds__(256, 3) sepfilter_tiled_kernel(const __grid_co
       float* tile = tiles + s * TILE_FLOATS;
       tma::mbar_wait(&full[s], (n >> 1) & 1);
 
-      if (BORDER != KB200_CONSTANT) {
-        const int ox = tx * TW - SEPT_XPAD, oy = y0 - HALO;
-        if (ox < 0 || oy < 0 || ox + BW > p.W || oy + BH > p.H) {  // CTA-uniform: the box sticks out of the image
-          for (int e = tid; e < BH * BW; e += 256) {
-            const int r = e / BW, c = e - r * BW;
-            const int gy = oy + r, gx = ox + c;
-            if ((unsigned)gy < (unsigned)p.H && (unsigned)gx < (unsigned)p.W) continue;
-            const int sr = border_index<BORDER>(gy, p.H) - oy, sc = border_index<BORDER>(gx, p.W) - ox;
-            // the folded source of every cell an output of this tile needs lies inside the box; cells
-            // further out (only reachable through the 8-texel alignment padding) are never read
-            if ((unsigned)sr < (unsigned)BH && (unsigned)sc < (unsigned)BW) tile[e] = tile[sr * BW + sc];
-          }
-          __syncthreads();
-        }
-      }
+      patch_box_border<BORDER>(tile, BH, BW, tx * TW - SEPT_XPAD, y0 - HALO, p);
 
       // ------------------------------------------------------------ row pass: tile -> mid
       {
@@ -182,7 +140,7 @@ __global__ void __launch_bounds__(256, 3) sepfilter_tiled_kernel(const __grid_co
         }
       }
       __syncthreads();  // mid complete, tile[s] no longer needed
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
 
       // ------------------------------------------------------------ column pass: mid -> out
       {

@@ -1,4 +1,5 @@
 // kornia_b200 -- host side of the band-walking SSIM kernel (ssim_vwalk.cuh).
+#include "persistent_launch.cuh"
 #include "ssim_vwalk.cuh"
 
 namespace kb200 {
@@ -7,16 +8,9 @@ template <int K>
 static int launch_ssimv(const CUtensorMap maps[4], const SsimVParams& p, cudaStream_t st) {
   auto kern = ssim_vwalk_kernel<K>;
   static unsigned long long configured = 0;
-  KB_SET_SMEM_ONCE(configured, kern, ssimv_smem_bytes<K>());const long long nbands = (long long)p.planes * ceil_div(p.W, SSIMV_TW);
-  const long long cap = 2ll * sm_count();
-  const int grid = (int)(nbands < cap ? nbands : cap);
-  kern<<<grid, 256, ssimv_smem_bytes<K>(), st>>>(maps[0], maps[1], maps[2], maps[3], p);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("ssim_vwalk launch failed: %s", cudaGetErrorString(e));
-    return KB200_ECUDA;
-  }
-  return KB200_OK;
+  KB_SET_SMEM_ONCE(configured, kern, ssimv_smem_bytes<K>());
+  kern<<<capped_grid((long long)p.planes * ceil_div(p.W, VWALK_TW), 2), 256, ssimv_smem_bytes<K>(), st>>>(maps[0], maps[1], maps[2], maps[3], p);
+  return launch_status("ssim_vwalk");
 }
 
 int ssim_vwalk_forward(const float* a, const float* b, const float* taps, float* out, int planes, int H, int W, int K, float C1, float C2,
@@ -25,20 +19,10 @@ int ssim_vwalk_forward(const float* a, const float* b, const float* taps, float*
   if ((W % 4) != 0 || (reinterpret_cast<uintptr_t>(a) & 15) != 0 || (reinterpret_cast<uintptr_t>(b) & 15) != 0 ||
       (reinterpret_cast<uintptr_t>(out) & 7) != 0)
     return KB200_EUNSUPPORTED;
-  if ((long long)planes * ceil_div(W, SSIMV_TW) > 0x7fffffffll) return KB200_EUNSUPPORTED;
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
+  if ((long long)planes * ceil_div(W, VWALK_TW) > 0x7fffffffll) return KB200_EUNSUPPORTED;
   CUtensorMap maps[4];  // main a, main b, prologue a, prologue b
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)planes};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  for (int i = 0; i < 4; ++i) {
-    const cuuint32_t box[3] = {(cuuint32_t)SSIMV_BW, (cuuint32_t)(i < 2 ? SSIMV_TH : K - 1), 1};
-    const float* src = (i & 1) ? b : a;
-    if (encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
+  for (int i = 0; i < 4; ++i)
+    if (!encode_plane_map(&maps[i], (i & 1) ? b : a, planes, H, W, VWALK_BW, i < 2 ? VWALK_TH : K - 1)) return KB200_EUNSUPPORTED;
   SsimVParams p{taps, out, planes, H, W, C1, C2, eps};
   switch (K) {
     case 3: return launch_ssimv<3>(maps, p, st);

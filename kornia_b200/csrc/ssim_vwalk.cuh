@@ -16,17 +16,11 @@
 // Launched by ssim_vwalk.cu; tests/test_variants_gpu.py checks it against the golden vectors, tools/hostemu bit for bit
 // against the scalar form.
 #pragma once
-#include "sepfilter_tiled.cuh"
-#include "filter_generic.cuh"
+#include "vwalk.cuh"
 
 namespace kb200 {
 
 constexpr int SSIM_MAX_K = 11;  // odd Gaussian windows up to 11 taps (the reference's default window)
-
-constexpr int SSIMV_TW = 64;
-constexpr int SSIMV_TH = 32;
-constexpr int SSIMV_XPAD = 8;
-constexpr int SSIMV_BW = SSIMV_TW + 2 * SSIMV_XPAD;  // 80
 
 struct SsimVParams {
   const float* taps;  // (K,) device
@@ -37,7 +31,7 @@ struct SsimVParams {
 
 template <int K>
 constexpr size_t ssimv_smem_bytes() {
-  return (size_t)(2 * 2 * SSIMV_TH * SSIMV_BW + 5 * (SSIMV_TH + K - 1) * SSIMV_TW) * sizeof(float) + 2 * sizeof(uint64_t);
+  return (size_t)(2 * 2 * VWALK_TH * VWALK_BW + 5 * (VWALK_TH + K - 1) * VWALK_TW) * sizeof(float) + 2 * sizeof(uint64_t);
 }
 
 template <int K>
@@ -46,20 +40,16 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
                                                             const __grid_constant__ SsimVParams p) {
   static_assert(K % 2 == 1 && K >= 3 && K <= SSIM_MAX_K, "odd windows up to 11 taps");
   constexpr int HALO = K / 2, CARRY = K - 1;
-  constexpr int TW = SSIMV_TW, TH = SSIMV_TH, BW = SSIMV_BW;
+  constexpr int TW = VWALK_TW, TH = VWALK_TH, BW = VWALK_BW;
   constexpr int MH = TH + CARRY;                 // rows of a row-filtered plane: image rows t*TH - HALO ... + MH
-  constexpr int COL0 = SSIMV_XPAD - HALO;        // box column of the first window position of output x = 0
+  constexpr int COL0 = VWALK_XPAD - HALO;        // box column of the first window position of output x = 0
   constexpr int A0 = COL0 & 3;
   constexpr int WIN = 4 + K - 1;                 // window positions feeding 4 neighbouring outputs
   constexpr int NV = (A0 + WIN + 3) / 4;         // aligned float4 loads per window
   constexpr int IMG_FLOATS = TH * BW;            // one image's box
   constexpr int SLOT_FLOATS = 2 * IMG_FLOATS;    // a slot holds the boxes of both images
   constexpr uint32_t TILE_BYTES = SLOT_FLOATS * 4, PRO_BYTES = 2 * CARRY * BW * 4;
-  constexpr int QUADS = TW / 4;                  // 16 quads per row
-  constexpr int RPS = 256 / QUADS;               // 16 rows per sweep of the CTA
-  constexpr int SWEEPS = TH / RPS;               // 2
-  constexpr int RY = 4;                          // rows per thread in the column pass
-  static_assert((TW / 2) * (TH / RY) == 256 && SWEEPS * RPS == TH && CARRY <= RPS, "thread mapping");
+  constexpr int QUADS = VWALK_QUADS, RPS = VWALK_RPS, SWEEPS = VWALK_SWEEPS, RY = VWALK_RY;
   static_assert((COL0 & ~3) + 4 * (QUADS - 1) + 4 * NV <= BW, "window loads stay inside a box row");
 
   extern __shared__ __align__(128) unsigned char ssimv_smem[];
@@ -68,55 +58,22 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
   uint64_t* full = reinterpret_cast<uint64_t*>(mid + 5 * MH * TW);  // [2]
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    tma::mbar_init(&full[0], 1);
-    tma::mbar_init(&full[1], 1);
-    tma::fence_barrier_init();
-  }
-  __syncthreads();
+  feed_init(full);
 
   const int bands = ceil_div(p.W, TW), tiles_y = ceil_div(p.H, TH);
   const Segments segs(p.planes * bands, tiles_y);
 
-  // box sequence of a band segment [t0, t1): prologue (t = t0 - 1), tile t0, ..., tile t1 - 1; issued two boxes ahead
-  struct Ahead {
-    int seg, strip, t0, t1, cursor, t, n;
-    bool live;
-  } ah{0, 0, 0, 0, 0, 0, 0, false};
-  auto ahead_next = [&]() {
-    if (ah.live && ah.t + 1 < ah.t1) {
-      ++ah.t;
-      ++ah.n;
-      return;
-    }
-    const bool first = !ah.live && ah.n == 0 && ah.seg == 0;
-    ah.live = segs.get(ah.seg, ah.strip, ah.t0, ah.t1, ah.cursor);
-    ++ah.seg;
-    ah.t = ah.t0 - 1;
-    if (!first) ++ah.n;
+  // box sequence of a band segment [t0, t1): prologue (t = t0 - 1), tile t0, ..., tile t1 - 1
+  TileFeed<true> feed(segs);
+  auto load = [&](int slot, int strip, int t, bool prologue) {
+    const int plane = strip / bands, band = strip - plane * bands;
+    float* dst = slots + slot * SLOT_FLOATS;
+    const int y = prologue ? (t + 1) * TH - HALO : t * TH + HALO;  // the prologue: the K - 1 rows above tile t + 1
+    tma::mbar_arrive_expect_tx(&full[slot], prologue ? PRO_BYTES : TILE_BYTES);
+    tma::load_3d(dst, prologue ? &pro_a : &map_a, &full[slot], band * TW - VWALK_XPAD, y, plane);
+    tma::load_3d(dst + IMG_FLOATS, prologue ? &pro_b : &map_b, &full[slot], band * TW - VWALK_XPAD, y, plane);
   };
-  auto issue = [&]() {
-    if (!ah.live) return;
-    const int plane = ah.strip / bands, band = ah.strip - plane * bands;
-    const int s = ah.n & 1;
-    float* slot = slots + s * SLOT_FLOATS;
-    tma::fence_proxy_async();
-    if (ah.t < ah.t0) {
-      tma::mbar_arrive_expect_tx(&full[s], PRO_BYTES);
-      tma::load_3d(slot, &pro_a, &full[s], band * TW - SSIMV_XPAD, ah.t0 * TH - HALO, plane);
-      tma::load_3d(slot + IMG_FLOATS, &pro_b, &full[s], band * TW - SSIMV_XPAD, ah.t0 * TH - HALO, plane);
-    } else {
-      tma::mbar_arrive_expect_tx(&full[s], TILE_BYTES);
-      tma::load_3d(slot, &map_a, &full[s], band * TW - SSIMV_XPAD, ah.t * TH + HALO, plane);
-      tma::load_3d(slot + IMG_FLOATS, &map_b, &full[s], band * TW - SSIMV_XPAD, ah.t * TH + HALO, plane);
-    }
-    ahead_next();
-  };
-  if (tid == 0) {
-    ahead_next();
-    issue();
-    issue();
-  }
+  if (tid == 0) feed.start(load);
 
   float k[K];
 #pragma unroll
@@ -129,7 +86,7 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
   int n = 0, strip, t0, t1, cursor = 0;
   for (int seg = 0; segs.get(seg, strip, t0, t1, cursor); ++seg) {
     const int plane = strip / bands, band = strip - plane * bands;
-    const int x0 = band * TW, ox = x0 - SSIMV_XPAD;
+    const int x0 = band * TW, ox = x0 - VWALK_XPAD;
     const int nl = ox < 0 ? -ox : 0;                    // box columns [0, nl) lie left of the image
     const int nr = ox + BW > p.W ? ox + BW - p.W : 0;   // box columns [BW - nr, BW) lie right of it
     const size_t base = (size_t)plane * p.H * p.W;
@@ -193,42 +150,16 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
         }
       }
       __syncthreads();  // rows written, boxes consumed
-      if (tid == 0) issue();
+      if (tid == 0) feed.issue(load);
       if (pro) continue;
 
       const int y0 = t * TH, gy0 = y0 - HALO;  // gy0: image row of mid row 0
-      if (gy0 < 0 || gy0 + MH > p.H) {         // CTA-uniform: first / last tiles of the band -- reflect row-filtered rows
-        for (int e = tid; e < MH * QUADS; e += 256) {
-          const int mr = e / QUADS, qd = e - mr * QUADS;
-          const int gy = gy0 + mr;
-          if ((unsigned)gy < (unsigned)p.H) continue;
-          const int sr = border_index<KB200_REFLECT>(gy, p.H) - gy0;  // an in-image row: never written by this loop
-          if ((unsigned)sr < (unsigned)MH) {
-#pragma unroll
-            for (int q = 0; q < 5; ++q) mid4[(q * MH + mr) * QUADS + qd] = mid4[(q * MH + sr) * QUADS + qd];
-          }
-        }
-        __syncthreads();
-      }
+      vwalk_reflect_rows<5, K>(mid4, gy0, p.H);  // first / last tiles of the band
 
       // ------------------------------------------------------------ column pass + index
       {
         float2 acc[5][RY];
-#pragma unroll
-        for (int q = 0; q < 5; ++q)
-#pragma unroll
-          for (int o = 0; o < RY; ++o) acc[q][o] = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < RY + K - 1; ++i) {
-#pragma unroll
-          for (int q = 0; q < 5; ++q) {
-            const float2 v = *reinterpret_cast<const float2*>(mid + (q * MH + rg * RY + i) * TW + 2 * cp);
-#pragma unroll
-            for (int o = 0; o < RY; ++o) {
-              if (i - o >= 0 && i - o < K) acc[q][o] = fma2_rn(make_float2(k[i - o], k[i - o]), v, acc[q][o]);
-            }
-          }
-        }
+        vwalk_column_pass<5, K>(mid, k, cp, rg, acc);
         const int gx = x0 + 2 * cp;
         if (gx < p.W) {  // W % 4 == 0: whole pairs
 #pragma unroll
@@ -254,18 +185,7 @@ __global__ void __launch_bounds__(256, 2) ssim_vwalk_kernel(const __grid_constan
         }
       }
       __syncthreads();  // every read of mid is done
-      if (t + 1 < t1) {
-        // carry rows [TH, MH) -> [0, CARRY) of all five planes: thread (rq, rr) moves exactly the cells it overwrites in
-        // the next row pass (mid row CARRY + rr + 16*it, quad rq)
-#pragma unroll
-        for (int it = 0; it < SWEEPS; ++it) {
-          const int R = CARRY + rr + it * RPS;
-          if (R >= TH) {
-#pragma unroll
-            for (int q = 0; q < 5; ++q) mid4[(q * MH + R - TH) * QUADS + rq] = mid4[(q * MH + R) * QUADS + rq];
-          }
-        }
-      }
+      if (t + 1 < t1) vwalk_carry_rows<5, K>(mid4, rq, rr);
     }
   }
 }

@@ -13,29 +13,11 @@ int warp_tma_backward(const float* gout, const float* src, const float* m, const
     return KB200_EUNSUPPORTED;
   if ((long long)B * C > 0x7fffffffll || (long long)B * ceil_div(h, 32) > 0x7fffffffll) return KB200_EUNSUPPORTED;
   if ((w & 1) != 0 || (reinterpret_cast<uintptr_t>(gout) & 7) != 0) return KB200_EUNSUPPORTED;  // 8-byte loads of gout
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return KB200_EUNSUPPORTED;
-  const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B * C};
-  const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMap mgsrc;
-  {
-    const cuuint32_t box[3] = {72, BWD_SH, (cuuint32_t)C};
-    void* base = gsrc ? (void*)gsrc : (void*)const_cast<float*>(src);  // unused when gsrc is null, but must encode
-    if (encode(&mgsrc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
+  CUtensorMap mgsrc;  // unused when gsrc is null, but must encode
+  if (!encode_plane_map(&mgsrc, gsrc ? gsrc : src, (long long)B * C, H, W, 72, BWD_SH, C)) return KB200_EUNSUPPORTED;
   CUtensorMap mgout;
-  {
-    const cuuint64_t odims[3] = {(cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)B * C};
-    const cuuint64_t ostrides[2] = {(cuuint64_t)w * 4, (cuuint64_t)h * w * 4};
-    const cuuint32_t box[3] = {64, 32, (cuuint32_t)C};
-    if ((w % 4) != 0 || (reinterpret_cast<uintptr_t>(gout) & 15) != 0 ||
-        encode(&mgout, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(gout), odims, ostrides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
+  if ((w % 4) != 0 || (reinterpret_cast<uintptr_t>(gout) & 15) != 0 || !encode_plane_map(&mgout, gout, (long long)B * C, h, w, 64, 32, C))
+    return KB200_EUNSUPPORTED;
   TmaBwdParams p{};
   p.gout = gout; p.src = src; p.m = m; p.bx = bx; p.by = by; p.gsrc = gsrc;
   p.B = B; p.H = H; p.W = W; p.h = h; p.w = w; p.Bm = Bm;
@@ -50,12 +32,7 @@ int warp_tma_backward(const float* gout, const float* src, const float* m, const
     p.record_batch = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + rows * TMA_CONSUMER_WARPS * 9 * sizeof(float));
   }
   CUtensorMap msrcwin;
-  {
-    const cuuint32_t box[3] = {72, BWD_SH, (cuuint32_t)C};
-    if (encode(&msrcwin, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return KB200_EUNSUPPORTED;
-  }
+  if (!encode_plane_map(&msrcwin, src, (long long)B * C, H, W, 72, BWD_SH, C)) return KB200_EUNSUPPORTED;
   if (dyn) {
     p.counter = take_work_counter(st);
     if (!p.counter) return KB200_EUNSUPPORTED;

@@ -62,17 +62,8 @@ struct TmaFwdArgs {
 // The source as (W, H, B * C) planes, one map per box height of warp_fwd_tma (tma_box_rows); false when the driver refuses.
 template <int BW, int BH>
 static bool encode_box_maps(TmaBoxMaps& maps, const TmaFwdArgs& a) {
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return false;
-  const cuuint64_t dims[3] = {(cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)a.B * a.C};
-  const cuuint64_t strides[2] = {(cuuint64_t)a.W * 4, (cuuint64_t)a.H * a.W * 4};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  for (int i = 0; i < TMA_BOX_HEIGHTS; ++i) {
-    const cuuint32_t box[3] = {(cuuint32_t)BW, (cuuint32_t)tma_box_rows(BH, i), 1};
-    if (encode(&maps.map[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(a.src), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return false;
-  }
+  for (int i = 0; i < TMA_BOX_HEIGHTS; ++i)
+    if (!encode_plane_map(&maps.map[i], a.src, (long long)a.B * a.C, a.H, a.W, BW, tma_box_rows(BH, i))) return false;
   return true;
 }
 

@@ -16,7 +16,7 @@
 #include <map>
 #include <vector>
 
-#include "../../kornia_b200/csrc/warp_tma.cuh"  // kb200::tma::EmuMap / EmuBar (tma_emu.inl)
+#include "../../kornia_b200/csrc/tma.cuh"  // kb200::tma::EmuMap / EmuBar (tma_emu.inl)
 
 uint3 threadIdx, blockIdx;
 dim3 blockDim, gridDim;

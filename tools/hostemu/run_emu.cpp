@@ -412,8 +412,8 @@ static void test_ssim(int planes, int H, int W, unsigned grid, bool lazy, int sp
   }
   float* o2 = aligned(o2s, n);
   {
-    const CUtensorMap ma = emu::make_map(a, W, H, planes, SSIMV_BW, SSIMV_TH, 1), mb = emu::make_map(b, W, H, planes, SSIMV_BW, SSIMV_TH, 1);
-    const CUtensorMap pa = emu::make_map(a, W, H, planes, SSIMV_BW, K - 1, 1), pb = emu::make_map(b, W, H, planes, SSIMV_BW, K - 1, 1);
+    const CUtensorMap ma = emu::make_map(a, W, H, planes, VWALK_BW, VWALK_TH, 1), mb = emu::make_map(b, W, H, planes, VWALK_BW, VWALK_TH, 1);
+    const CUtensorMap pa = emu::make_map(a, W, H, planes, VWALK_BW, K - 1, 1), pb = emu::make_map(b, W, H, planes, VWALK_BW, K - 1, 1);
     SsimVParams p{taps.data(), o2, planes, H, W, C1, C2, eps};
     emu::launch(grid, dim3(256), [&] { ssim_vwalk_kernel<K>(ma, mb, pa, pb, p); });
   }
@@ -1110,7 +1110,7 @@ static void test_corner(int planes, int C, int H, int W, bool diff, int specials
   prm.taps = g; prm.kptr = nullptr; prm.s4 = sigmas ? s4.data() : nullptr; prm.out = aligned(os, n);
   prm.planes = planes; prm.C = C; prm.H = H; prm.W = W; prm.k = k;
   for (int e = 0; e < 18; ++e) prm.st[e] = st[e];
-  const CUtensorMap map = emu::make_map(x, W, H, planes, SSIMV_BW, SSIMV_TH + 2, 1), pro = emu::make_map(x, W, H, planes, SSIMV_BW, CORNER_K - 1 + 2, 1);
+  const CUtensorMap map = emu::make_map(x, W, H, planes, VWALK_BW, VWALK_TH + 2, 1), pro = emu::make_map(x, W, H, planes, VWALK_BW, CORNER_K - 1 + 2, 1);
   emu::launch(grid, dim3(256), [&] { corner_vwalk_kernel<KIND>(map, pro, prm); });
   compare_bits_or_nan(std::string("corner_vwalk_kernel ") + (KIND == RESP_HARRIS ? "Harris" : "GFTT") + (diff ? " diff " : " sobel ") + std::to_string(planes) + "x" +
                    std::to_string(H) + "x" + std::to_string(W) + " C=" + std::to_string(C) + (sigmas ? " sigmas" : "") + (specials ? " special texels" : "") +
