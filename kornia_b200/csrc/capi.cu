@@ -47,9 +47,6 @@ static const struct {
     {OPT_U8_TILED, "u8_tiled", 1},
     {OPT_BWD_STRIDE1, "bwd_stride1", 1},
     {OPT_DYN_SCHED, "dyn_sched", 1},
-    {OPT_DYN_CHUNK, "dyn_chunk", 10},
-    {OPT_DYN_STATIC, "dyn_static", 85},
-    {OPT_SWEEP, "sweep", 1},
 };
 static_assert(sizeof(OPTIONS) / sizeof(OPTIONS[0]) == OPT_COUNT, "one OPTIONS row per Option");
 static int g_options[OPT_COUNT];

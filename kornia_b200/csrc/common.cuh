@@ -90,11 +90,10 @@ enum Option {
   OPT_U8_TILED,        // staged-window uint8 ingest warp (off: per-tap kernel)
   OPT_BWD_STRIDE1,     // tiled backward on stride-1 lanes (default; 0: the column-pair lanes, dealt out in advance).  At cfg4
                        // the column pairs were 5 % slower on a B200; on an H100 SXM at 400 W, one alternated A/B had them
-                       // 2.6 % faster (4.69 vs 4.81 ms per launch).  The default has not been chosen again.
-  OPT_DYN_SCHED,       // headline warp: strips handed out at run time in chunks (off: dealt out in advance)
-  OPT_DYN_CHUNK,       // tiles per chunk of the run-time work distribution (forward kernel)
-  OPT_DYN_STATIC,      // percent of the full rounds of strips still dealt out in advance by the DYN forward kernel
-  OPT_SWEEP,           // DYN forward kernel: every run of tiles drawn in raster order (off: the strip deal of dyn_chunk / dyn_static)
+                       // 2.6 % faster (4.69 vs 4.81 ms per launch).  On an H100 SXM at 700 W, 4 alternated runs each of
+                       // bench.py --workload warp_bwd (kernel ms, median): default 4.78, bwd_stride1=0 4.66, dyn_sched=0
+                       // (stride-1 lanes, static deal) 4.63: the default's deficit is the run-time deal's, not the lanes'.
+  OPT_DYN_SCHED,       // warp forward and backward: work handed out at run time (off: dealt out in advance)
   OPT_COUNT
 };
 int option(Option o);

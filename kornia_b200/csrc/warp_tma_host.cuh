@@ -9,8 +9,8 @@ constexpr int TMA_L2_PROMO = 256;  // 256-B L2 promotion on the tensor map (not 
 
 // 64 x 32 output tiles, 72-wide source boxes of 33 to 40 rows, 2 stages, 2 CTAs per SM: not compared with 3 stages, 96-wide
 // boxes or other tiles on the H100.  On an H100 SXM (700 W) the headline launch ran at 0.77 of the 3.35 TB/s roofline under
-// the strip deal (4.95 ms; 5.36 ms with the 40-row box for every tile).  DYN launches run the sweep by default (every tile
-// drawn in raster order): on an H100 held to 400 W, 4.47-4.55 ms against 4.95-4.97 ms for the strip deal.  Column-wise walks
+// the strip deal (4.95 ms; 5.36 ms with the 40-row box for every tile).  DYN launches run the sweep (every tile drawn in
+// raster order): on an H100 held to 400 W, 4.47-4.55 ms against 4.95-4.97 ms for the strip deal it replaced.  Column-wise walks
 // of bands of strips were measured and lost (DESIGN.md 4.1).
 template <int NC, int INTERP, int PAD, bool PROJ, bool ALIGN, int TW = 64, int TH = 32, int BW = 72, int BH = 40, int NSTAGE = 2, bool DYN = false>
 static int launch_warp_tma(const TmaBoxMaps& maps, const TmaWarpParams& p, cudaStream_t st, int ctas_per_sm = 2) {
@@ -25,13 +25,6 @@ static int launch_warp_tma(const TmaBoxMaps& maps, const TmaWarpParams& p, cudaS
     TmaWarpParams q = p;
     q.counter = take_work_counter(st);
     if (!q.counter) return KB200_EUNSUPPORTED;
-    if (option(OPT_SWEEP)) {  // every run drawn, in raster order (warp_fwd_tma: the producer)
-      q.chunk_tiles = SWEEP_TILES;
-      q.static_pct = 0;
-    } else {
-      q.chunk_tiles = option(OPT_DYN_CHUNK) > 0 ? option(OPT_DYN_CHUNK) : 10;
-      q.static_pct = option(OPT_DYN_STATIC);
-    }
     kern<<<grid, TMA_THREADS, smem, st>>>(maps, q);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
@@ -71,7 +64,7 @@ template <int INTERP>
 static int warp_tma_forward_impl(const TmaFwdArgs& a, cudaStream_t st) {
   TmaBoxMaps map;
   if (!encode_box_maps<72, 40>(map, a)) return KB200_EUNSUPPORTED;
-  TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr, 0, 0};
+  TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr};
   const int C = a.C, pad = a.pad;
   const bool projective = a.projective != 0, align = a.align != 0;
   // run-time work distribution (warp_fwd_tma<DYN>) for bilinear RGB batches with enough strips to go round several times

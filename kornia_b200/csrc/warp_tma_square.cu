@@ -23,7 +23,7 @@ int warp_tma_forward_square(const TmaFwdArgs& a, cudaStream_t st) {
   if (a.C != 1 && a.C != 3) return KB200_EUNSUPPORTED;
   TmaBoxMaps map;
   if (!encode_box_maps<SQ_BW, SQ_BH>(map, a)) return KB200_EUNSUPPORTED;
-  const TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr, 0, 0};
+  const TmaWarpParams p{a.src, a.m, a.bx, a.by, a.fill, a.out, a.B, a.H, a.W, a.h, a.w, a.Bm, a.align, a.only_class, nullptr};
   const bool projective = a.projective != 0, align = a.align != 0;
 #define KB_SQ_CASE(NC_, PAD_) \
   if (a.C == NC_ && a.pad == PAD_) return launch_square<NC_, PAD_>(map, p, projective, align, st);

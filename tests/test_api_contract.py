@@ -187,10 +187,15 @@ def test_kernel_selection_switches_agree_everywhere():
         assert lib.kb200_get_option(name.encode()) == before
     assert lib.kb200_get_option(b"no_such_switch") == int_min
     assert lib.kb200_set_option(b"no_such_switch", 1) != 0
-    config.set("dyn_chunk", 7)
-    assert config.get("dyn_chunk") == 7 and lib.kb200_get_option(b"dyn_chunk") == 7
+    config.set("dyn_sched", 0)
+    assert config.get("dyn_sched") == 0 and lib.kb200_get_option(b"dyn_sched") == 0
     config.reset()
-    assert config.get("dyn_chunk") == 10 and config.get("dyn_sched") == 1 and config.get("dyn_static") == 85
+    assert config.get("dyn_sched") == 1
+    for name in ("sweep", "dyn_chunk", "dyn_static"):  # removed switches are unknown names
+        assert lib.kb200_set_option(name.encode(), 1) != 0, name
+        assert lib.kb200_get_option(name.encode()) == int_min, name
+        with pytest.raises(KeyError):
+            config.set(name, 1)
 
 
 def test_c_abi_version_and_error_channel():

@@ -1,7 +1,7 @@
-"""The sweep of the headline forward kernel (warp_fwd_tma<DYN>, switch sweep): every run of tiles drawn from one counter in raster
-order.  Only who takes which tile changes, so the output must equal, bit for bit, the strip deal (sweep=0) and the generic kernel,
-and every pixel must be written exactly once -- also at sizes that leave partial strips and partial tiles, with samples of the
-other footprint class that the wide kernel skips, and inside a CUDA graph."""
+"""The sweep of the headline forward kernel (warp_fwd_tma<DYN>): every run of tiles drawn from one counter in raster order.  Only
+who takes which tile changes, so the output must equal, bit for bit, the static deal (dyn_sched=0) and the generic kernel, and
+every pixel must be written exactly once -- also at sizes that leave partial strips and partial tiles, with samples of the other
+footprint class that the wide kernel skips, and inside a CUDA graph."""
 import pytest
 import torch
 
@@ -41,19 +41,19 @@ def batch():
 
 @pytest.mark.parametrize("pad", ["zeros", "border", "reflection", "fill"])
 @pytest.mark.parametrize("projective", [True, False])
-def test_sweep_bit_identical_to_strip_deal_and_generic(batch, pad, projective):
+def test_sweep_bit_identical_to_static_deal_and_generic(batch, pad, projective):
     src, M = batch
     if not projective:
         M = M[:, :2].contiguous()
     fill = torch.tensor([0.2, 0.5, 0.8], device=DEV) if pad == "fill" else None
-    assert K.config.get("sweep") == 1 and K.config.get("dyn_sched") == 1
+    assert K.config.get("dyn_sched") == 1
     for dsize in ((H, W), (1000, 1900)):  # 1000 x 1900: a partial last strip and a partial last tile in every strip
         for align in (True, False):
             run = lambda: _forward_into_nan(src, M, dsize, projective, pad, align, fill)  # noqa: E731
             sweep = run()
             assert _lib.last_warp_variant() == "tma_tile"
             assert not torch.isnan(sweep).any(), (dsize, align, "a pixel was not written")
-            with K.config.override(sweep=0):
+            with K.config.override(dyn_sched=0):
                 deal = run()
             with K.config.override(tma=0):
                 gen = run()
@@ -66,9 +66,9 @@ def test_sweep_inside_a_cuda_graph():
     """The launch zeroes its work counter on its stream, which a capture records: replays start from zero."""
     many = torch.rand(400, 3, 96, 192, device=DEV)  # 1 200 strips of three tiles
     Mm = _bench_homographies(400, 96, 192, 5).to(DEV)
-    with K.config.override(dyn_sched=0):
+    with K.config.override(tma=0):
         want = K.warp_perspective(many, Mm, (96, 192))
-    with K.config.override(sweep=0):
+    with K.config.override(dyn_sched=0):
         deal = K.warp_perspective(many, Mm, (96, 192))
     assert torch.equal(deal, want)
     graphed = K.graphs.GraphedCall(lambda a, b: K.warp_perspective(a, b, (96, 192)), many, Mm)

@@ -24,7 +24,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=256)
 ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--steps", type=int, default=20)
-ap.add_argument("arms", nargs="*", default=["default", "sweep=0", "dyn_sched=0", "copy"])
+ap.add_argument("arms", nargs="*", default=["default", "dyn_sched=0", "copy"])
 args = ap.parse_args()
 
 try:
