@@ -318,6 +318,23 @@ int kb200_patch_orientation_forward(const void* x, const void* weighting, const 
                                     long long sH, int num_ang_bins, float eps, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * LAF patch extraction (feature/laf.py extract_patches_from_pyramid / extract_patches_simple) in ONE kernel per call:
+ * each patch picks its pyramid level, maps its PS x PS grid and samples every channel bilinearly with 'border' padding,
+ * writing B * N * C * PS * PS floats once, instead of about 25 ATen kernels per (level, image) over all N patches.
+ *   levels      n_levels pointers to fp32 (B_l, C, h_l, w_l) levels with column stride 1 (level 0 the image, then pyrdowns)
+ *   level_dims  5 per level: h, w and the batch, channel and row element strides
+ *   laf         contiguous fp32 (B, N, 2, 3); B <= every level's batch
+ *   base        contiguous fp32 PS base-grid coordinates (affine_grid, align_corners=False)
+ *   out         contiguous fp32 (B, N, C, PS, PS)
+ * select_level = 0 samples level 0 only (extract_patches_simple).  A patch whose level is not among the n_levels given
+ * (1 <= n_levels <= 32) is written as zeros.  Each output element is written once and depends on its patch only.
+ * B * N = 0 launches nothing.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_extract_patches_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                                  void* out, long long B, long long N, int C, int PS, int normalize, int select_level, int dtype,
+                                  void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

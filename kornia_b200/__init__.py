@@ -29,7 +29,9 @@ def install(kornia_module=None) -> None:
     imported ``kornia`` package.  A defining module the package lacks, or a name its module does not define, is skipped.
     The per-keypoint stages of the SIFT-style pipelines are rebound too: ``SIFTDescriptor`` / ``sift_describe`` and
     ``PatchDominantGradientOrientation``, which ``SIFTFeature``, ``SIFTFeatureScaleSpace`` and the ``LAFOrienter``
-    constructor build by name.  Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``,
+    constructor build by name, and the patch extraction ``extract_patches_from_pyramid`` / ``extract_patches_simple``
+    that ``get_laf_descriptors`` / ``LAFDescriptor``, ``LAFOrienter`` and the affine shape estimators call by name (so
+    those reach the fused extraction at call time, whenever they were built).  Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``,
     ``MultiResolutionDetector``, ``SIFTFeature``, ``SIFTFeatureScaleSpace`` or ``LAFOrienter`` built before ``install()``
     keeps the reference pyramid, ``NonMaximaSuppression2d``, sub-pixel refiner, descriptor and orienter it holds.
 
@@ -85,6 +87,10 @@ def install(kornia_module=None) -> None:
         "SIFTDescriptor": ("feature.siftdesc", feature.SIFTDescriptor),
         "sift_describe": ("feature.siftdesc", feature.sift_describe),
         "PatchDominantGradientOrientation": ("feature.orientation", feature.PatchDominantGradientOrientation),
+        # get_laf_descriptors / LAFDescriptor (integrated.py), LAFOrienter (orientation.py) and the affine shape estimators
+        # (affine_shape.py) import these by name and call them at call time
+        "extract_patches_from_pyramid": ("feature.laf", feature.extract_patches_from_pyramid),
+        "extract_patches_simple": ("feature.laf", feature.extract_patches_simple),
     }
     originals = {}
     for name, (mod, fn) in defining.items():

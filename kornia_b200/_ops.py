@@ -951,6 +951,76 @@ _define("patch_orientation_fwd", "(Tensor x, Tensor weighting, Tensor smooth, in
         lambda x, weighting, smooth, num_ang_bins, eps: (_check_orientation_args(x, weighting, smooth, num_ang_bins), x.new_empty((x.shape[0],)))[1])
 
 
+_PATCH_MAX_LEVELS = 32  # the kernel's level table (csrc/laf_patches.cuh)
+
+
+def _check_patch_levels(levels, laf, PS: int, select_level: bool) -> None:
+    """What the patch extraction kernel reads: 1..32 fp32 (B_l, C, h_l, w_l) levels of one batch and channel count, each
+    the halving (h // 2, w // 2) of the one before, with a batch of at least the LAFs'; fp32 (B, N, 2, 3) LAFs on the same
+    device; PS >= 1.  Without level selection exactly one level (the image)."""
+    if len(levels) < 1 or len(levels) > _PATCH_MAX_LEVELS or (not select_level and len(levels) != 1):
+        raise RuntimeError(f"kornia_b200: expected 1..{_PATCH_MAX_LEVELS} pyramid levels (1 without level selection), got {len(levels)}")
+    if laf.dim() != 4 or tuple(laf.shape[2:]) != (2, 3):
+        raise RuntimeError(f"kornia_b200: expected (B, N, 2, 3) LAFs, got {tuple(laf.shape)}")
+    if PS < 1:
+        raise RuntimeError(f"kornia_b200: bad patch size {PS}")
+    x0 = levels[0]
+    for l, x in enumerate(levels):
+        if x.dim() != 4:
+            raise RuntimeError(f"kornia_b200: pyramid level {l} must be (B, C, H, W), got {tuple(x.shape)}")
+        if x.shape[0] != x0.shape[0] or x.shape[1] != x0.shape[1]:
+            raise RuntimeError(f"kornia_b200: pyramid level {l} {tuple(x.shape)} does not share level 0's batch and channels {tuple(x0.shape[:2])}")
+        if l > 0 and (x.shape[2] != levels[l - 1].shape[2] // 2 or x.shape[3] != levels[l - 1].shape[3] // 2):
+            raise RuntimeError(f"kornia_b200: pyramid level {l} {tuple(x.shape[2:])} is not the halving of level {l - 1} "
+                               f"{tuple(levels[l - 1].shape[2:])}")
+        _fake_same_device(laf, x)
+        _same(x0, x, f"pyramid level {l}")
+    if x0.shape[0] < laf.shape[0]:
+        raise RuntimeError(f"kornia_b200: {laf.shape[0]} LAF sets for {x0.shape[0]} images")
+    _fake_same_device(x0, laf)
+    _same(x0, laf, "the LAFs")
+
+
+def _affine_base(PS: int, device) -> torch.Tensor:
+    """affine_grid's base coordinates (align_corners=False) as ATen builds them on ``device``: linspace(-1, 1, PS) *
+    (PS - 1) / PS, or 0 for PS = 1.  Built once per (PS, device) with those torch ops, so they are ATen's values bit for bit."""
+    from .geometry._prelude import _cached
+
+    def build():
+        if PS <= 1:
+            return torch.zeros(1, device=device)
+        return torch.linspace(-1, 1, PS, device=device) * (PS - 1) / PS
+
+    return _cached(("laf_patch_base", PS, str(device)), build)
+
+
+def _extract_patches_cuda(levels, laf, PS, normalize, select_level):
+    """(B, N, C, PS, PS) patches at the LAFs ``laf`` (B, N, 2, 3), sampled from ``levels`` (the image, then its pyrdowns)."""
+    _require_cuda(laf, "the LAFs")
+    _check_patch_levels(levels, laf, PS, select_level)
+    B, N, C = laf.shape[0], laf.shape[1], levels[0].shape[1]
+    out = torch.empty((B, N, C, PS, PS), device=laf.device, dtype=laf.dtype)
+    if B * N == 0:
+        return out
+    lv = [x if x.shape[-1] == 1 or x.stride(-1) == 1 else x.contiguous() for x in levels]
+    lafc = laf.contiguous()
+    base = _affine_base(PS, laf.device)
+    ptrs = (ctypes.c_void_p * len(lv))(*[x.data_ptr() for x in lv])
+    dims = (ctypes.c_longlong * (5 * len(lv)))(*[v for x in lv for v in (x.shape[2], x.shape[3], x.stride(0), x.stride(1),
+                                                                         x.stride(2) if x.shape[2] > 1 else x.shape[3])])
+    with torch.cuda.device(laf.device), _Timed("extract_patches_forward", laf):
+        _lib.call("kb200_extract_patches_forward", ptrs, dims, len(lv), _ptr(lafc), _ptr(base), _ptr(out), B, N, C, PS, int(normalize),
+                  int(select_level), _dtype_code(laf), _stream(laf))
+    _bump()
+    return out
+
+
+_define("extract_patches_fwd", "(Tensor[] levels, Tensor laf, int PS, bool normalize, bool select_level) -> Tensor", _extract_patches_cuda,
+        lambda levels, laf, PS, normalize, select_level: (_check_patch_levels(levels, laf, PS, select_level),
+                                                          laf.new_empty((laf.shape[0], laf.shape[1], levels[0].shape[1], PS, PS)))[1],
+        first_tensor="the LAFs")
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -1129,5 +1199,5 @@ OPERATORS: Tuple[str, ...] = (
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
     "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd", "quad_interp3d_fwd", "sift_describe_fwd",
-    "patch_orientation_fwd",
+    "patch_orientation_fwd", "extract_patches_fwd",
 )

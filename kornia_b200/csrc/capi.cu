@@ -708,6 +708,24 @@ int kb200_patch_orientation_forward(const void* x, const void* weighting, const 
   return rc;
 }
 
+namespace kb200 {
+// laf_patches.cu (its kernel is not a template, so its header is included there only)
+int extract_patches_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                            void* out, long long B, long long N, int C, int PS, int normalize, int select_level, cudaStream_t st);
+}  // namespace kb200
+
+int kb200_extract_patches_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                                  void* out, long long B, long long N, int C, int PS, int normalize, int select_level, int dtype,
+                                  void* stream) {
+  KB_CHECK_ARG(B >= 0 && N >= 0 && C > 0 && PS > 0, "bad sizes B=%lld N=%lld C=%d PS=%d", B, N, C, PS);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused patch extraction is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  return extract_patches_forward(levels, level_dims, n_levels, laf, base, out, B, N, C, PS, normalize, select_level, (cudaStream_t)stream);
+}
+
 int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void* kernel_y, void* out, int B, int C, int H, int W,
                                  int Bkx, int kw, int Bky, int kh, int border, int same, double weight, int dtype, void* stream) {
   int rc = check_filter(x, kernel_x, B, C, H, W, Bkx, kh, kw, border, same, dtype);

@@ -196,12 +196,16 @@ struct PixelSampler {
   T cx[NT], cy[NT];
   T inv_cover;
 
-  __device__ __forceinline__ void prepare(T ix, T iy, int H, int W_, bool align) {
+  __device__ __forceinline__ void prepare(T ix, T iy, int H, int W_, bool align) { prepare_rows(ix, iy, H, W_, W_, align); }
+
+  // Same, on a plane whose rows lie `row` elements apart (row >= W_): bounds and padding use the width W_, tap offsets the row
+  // stride.  prepare() is the contiguous case, row == W_.
+  __device__ __forceinline__ void prepare_rows(T ix, T iy, int H, int W_, int row, bool align) {
     using R = RN<T>;
-    W = W_;
+    W = row;
     inv_cover = T(0);
     if (INTERP == KB200_BILINEAR) {
-      ix = pad_coord<T, SPAD>(ix, W, align);
+      ix = pad_coord<T, SPAD>(ix, W_, align);
       iy = pad_coord<T, SPAD>(iy, H, align);
       const T x0f = R::floor(ix), y0f = R::floor(iy);
       const T x1f = R::add(x0f, T(1)), y1f = R::add(y0f, T(1));
@@ -209,8 +213,8 @@ struct PixelSampler {
       const T wy1 = R::sub(y1f, iy), wy0 = R::sub(iy, y0f);
       w[0] = R::mul(wx1, wy1); w[1] = R::mul(wx0, wy1); w[2] = R::mul(wx1, wy0); w[3] = R::mul(wx0, wy0);
       const int x0 = (int)x0f, y0 = (int)y0f;
-      ok[0] = in_bounds(y0, x0, H, W); ok[1] = in_bounds(y0, x0 + 1, H, W);
-      ok[2] = in_bounds(y0 + 1, x0, H, W); ok[3] = in_bounds(y0 + 1, x0 + 1, H, W);
+      ok[0] = in_bounds(y0, x0, H, W_); ok[1] = in_bounds(y0, x0 + 1, H, W_);
+      ok[2] = in_bounds(y0 + 1, x0, H, W_); ok[3] = in_bounds(y0 + 1, x0 + 1, H, W_);
       o = y0 * W + x0;
       if (PAD == KB200_FILL) {
         T cover = T(0);
@@ -220,10 +224,10 @@ struct PixelSampler {
         inv_cover = R::sub(T(1), cover);
       }
     } else if (INTERP == KB200_NEAREST) {
-      ix = pad_coord<T, SPAD>(ix, W, align);
+      ix = pad_coord<T, SPAD>(ix, W_, align);
       iy = pad_coord<T, SPAD>(iy, H, align);
       const int xn = (int)R::rint(ix), yn = (int)R::rint(iy);
-      ok[0] = in_bounds(yn, xn, H, W);
+      ok[0] = in_bounds(yn, xn, H, W_);
       o = yn * W + xn;
       if (PAD == KB200_FILL) inv_cover = ok[0] ? T(0) : T(1);
     } else {  // bicubic: coordinates stay un-padded, every tap is padded on its own
@@ -234,9 +238,9 @@ struct PixelSampler {
       for (int i = 0; i < NT; ++i) {
         // the tap coordinates as ATen's forward spells them: ix_nw - 1, ix_nw + 0, ix_nw + 1, ix_nw + 2 but iy_nw - 1 + i.  The
         // same values below 2^24; beyond it (fx - 1) + 2 and fx + 1 round differently, which 'reflection' folds to other texels.
-        const int xi = (int)pad_coord<T, SPAD>(R::add(fx, T(i - 1)), W, align);
+        const int xi = (int)pad_coord<T, SPAD>(R::add(fx, T(i - 1)), W_, align);
         const int yi = (int)pad_coord<T, SPAD>(R::add(R::sub(fy, T(1)), T(i)), H, align);
-        xok[i] = (unsigned)xi < (unsigned)W;
+        xok[i] = (unsigned)xi < (unsigned)W_;
         yok[i] = (unsigned)yi < (unsigned)H;
         xo[i] = xi;
         yo[i] = yi * W;

@@ -25,6 +25,7 @@ from torch import nn
 
 from ... import _lib, _ops, config
 from ...core.check import check, check_shape
+from .._prelude import _cached
 from ...filters.filter import filter2d, filter2d_separable
 from ...filters.gaussian import gaussian_blur2d
 
@@ -38,6 +39,17 @@ def _binomial5x5() -> torch.Tensor:
     reference's -- ``filter2d`` moves it to the image's device and dtype (filter.py:124-126)."""
     row = torch.tensor(_BINOMIAL)
     return (row[:, None] * row[None, :])[None] / 256.0
+
+
+def _binomial5x5_on(device, dtype) -> torch.Tensor:
+    """:func:`_binomial5x5` made once per (device, dtype) on that device (the same values: small integers over 256), so a
+    ``pyrdown`` call copies nothing from the host and can be captured in a CUDA graph."""
+
+    def build():
+        row = torch.tensor(_BINOMIAL, device=device)
+        return ((row[:, None] * row[None, :])[None] / 256.0).to(dtype)
+
+    return _cached(("binomial5x5", str(device), dtype), build)
 
 
 def _fused_request(input: torch.Tensor, border_type: str, align_corners: bool, factor: float):
@@ -54,7 +66,7 @@ def _fused_request(input: torch.Tensor, border_type: str, align_corners: bool, f
     code = _lib.BORDERS.get(str(border_type).lower())
     if code is None or code == _lib.CIRCULAR:
         return None
-    return _binomial5x5().to(device=input.device, dtype=input.dtype), code
+    return _binomial5x5_on(input.device, input.dtype), code
 
 
 def pyrdown(input: torch.Tensor, border_type: str = "reflect", align_corners: bool = False, factor: float = 2.0) -> torch.Tensor:
@@ -67,7 +79,7 @@ def pyrdown(input: torch.Tensor, border_type: str = "reflect", align_corners: bo
             return _ops.pyrdown_fused(input, *fused)
         except _lib.Unsupported:
             pass
-    blurred = filter2d(input, _binomial5x5(), border_type)
+    blurred = filter2d(input, _binomial5x5_on(input.device, input.dtype), border_type)
     size = (int(float(height) / factor), int(float(width) // factor))  # the reference's mixed / and // (pyramid.py:452)
     return F.interpolate(blurred, size=size, mode="bilinear", align_corners=align_corners)
 

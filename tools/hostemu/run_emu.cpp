@@ -20,6 +20,7 @@
 #include "../../kornia_b200/csrc/quad_interp.cuh"
 #include "../../kornia_b200/csrc/siftdesc.cuh"
 #include "../../kornia_b200/csrc/patch_orientation.cuh"
+#include "../../kornia_b200/csrc/laf_patches.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -1019,6 +1020,119 @@ static void test_orient(long long N, int P, int A, int specials, unsigned grid) 
   compare_bits_or_nan(what, got.data(), want.data(), got.size());
 }
 
+// Scalar restatement of extract_patches_from_pyramid / extract_patches_simple (kornia/feature/laf.py) in the kernel's op order
+// (csrc/laf_patches.cuh): normalisation, scale, level, the level's affine map, then ATen's bilinear 'border' grid_sample
+// written out tap by tap.  Levels are random planes of the halving shapes (their values do not matter to the kernel).
+static float bilinear_border(const float* s, int h, int w, int sH, float gx, float gy) {
+  float ix = (float)(fmaf(gx + 1.f, (float)w, -1.f) * 0.5f), iy = (float)(fmaf(gy + 1.f, (float)h, -1.f) * 0.5f);
+  ix = std::fmin((float)(w - 1), std::fmax(ix, 0.f));
+  iy = std::fmin((float)(h - 1), std::fmax(iy, 0.f));
+  const float x0 = floorf(ix), y0 = floorf(iy);
+  const float wx1 = (x0 + 1.f) - ix, wx0 = ix - x0, wy1 = (y0 + 1.f) - iy, wy0 = iy - y0;
+  const int xi = (int)x0, yi = (int)y0;
+  float acc = 0.f;
+  if (xi < w && yi < h) acc = fmaf(s[yi * sH + xi], wx1 * wy1, acc);
+  if (xi + 1 < w && yi < h) acc = fmaf(s[yi * sH + xi + 1], wx0 * wy1, acc);
+  if (xi < w && yi + 1 < h) acc = fmaf(s[(yi + 1) * sH + xi], wx1 * wy0, acc);
+  if (xi + 1 < w && yi + 1 < h) acc = fmaf(s[(yi + 1) * sH + xi + 1], wx0 * wy0, acc);
+  return acc;
+}
+
+static void test_patches(int B, long long N, int C, int h, int w, int PS, int n_levels, bool normalize, bool select, int row_pad, bool nonfinite,
+                         unsigned grid) {
+  std::vector<std::vector<float>> store(n_levels);
+  LafPatchParams p{};
+  int hl = h, wl = w;
+  for (int l = 0; l < n_levels; ++l, hl /= 2, wl /= 2) {
+    const int sH = wl + (l == 0 ? row_pad : 0);
+    const long long sC = (long long)sH * hl + (l == 0 ? 3 : 0), sB = sC * C + (l == 0 ? 7 : 0);
+    store[l] = randv((size_t)(sB * B), -1.f, 2.f);
+    p.lv[l] = LevelDesc{store[l].data(), sB, sC, hl, wl, sH};
+  }
+  std::vector<float> laf((size_t)(B * N * 6)), base(PS);
+  const int built_top = n_levels;
+  for (long long n = 0; n < B * N; ++n) {
+    const float u = randv(1, -1.5f, (float)built_top + 1.5f)[0], s = powf(2.f, u) * PS / 2.f, a = randv(1, 0.f, 6.2831853f)[0];
+    const float sh = randv(1, -0.3f, 0.3f)[0], r = randv(1, 0.6f, 1.6f)[0];
+    float* L = laf.data() + n * 6;
+    L[0] = s * cosf(a) * r; L[1] = s * (cosf(a) * sh - sinf(a) / r); L[2] = randv(1, -0.2f, 1.2f)[0] * (w - 1);
+    L[3] = s * sinf(a) * r; L[4] = s * (sinf(a) * sh + cosf(a) / r); L[5] = randv(1, -0.2f, 1.2f)[0] * (h - 1);
+    if (!normalize)
+      for (int k = 0; k < 6; ++k) L[k] /= (float)std::max(1, std::min(h, w) - 1);
+    if (nonfinite && n % 4 == 1) L[(n / 4) % 6] = (n % 8 == 1) ? NAN : ((n % 16 == 5) ? -INFINITY : INFINITY);
+  }
+  for (int j = 0; j < PS; ++j) base[j] = PS > 1 ? (-1.f + 2.f * j / (float)(PS - 1)) * (float)(PS - 1) / (float)PS : 0.f;
+  const size_t total = (size_t)(B * N * C * PS * PS);
+  std::vector<float> got(total, -777.f), want(total);
+  p.laf = laf.data();
+  p.base = base.data();
+  p.out = got.data();
+  p.N = N;
+  p.total = B * N;
+  p.C = C;
+  p.PS = PS;
+  p.n_levels = n_levels;
+  p.normalize = normalize;
+  p.select_level = select;
+  if (normalize) {
+    p.n_lin = 1.0f / (float)std::min(h - 1, w - 1);
+    p.n_tx = (float)(1.0 / (double)(w - 1));
+    p.n_ty = (float)(1.0 / (double)(h - 1));
+  }
+  p.max_clamp = (float)std::max(0, std::min(h, w) / PS - 1);
+  emu::launch(grid, dim3(LP_NT), [&] { laf_patches_kernel(p); });
+  for (long long n = 0; n < B * N; ++n) {
+    const float* L = laf.data() + n * 6;
+    float a = L[0], b = L[1], x = L[2], c = L[3], d = L[4], y = L[5];
+    if (normalize) {
+      a = p.n_lin * a; b = p.n_lin * b; x = p.n_tx * x; c = p.n_lin * c; d = p.n_lin * d; y = p.n_ty * y;
+    }
+    int lvl = 0;
+    if (select) {
+      const float m0 = (float)std::min(h - 1, w - 1);
+      const float det = ((m0 * a) * (m0 * d) - (m0 * c) * (m0 * b)) + 1e-10f;
+      const float sc = (2.0f * sqrtf(fabsf(det))) * (1.0f / (float)PS);
+      float l = log2f(sc);
+      if (l == l) l = std::fmin(std::fmax(l, 0.f), p.max_clamp);
+      const long long L64 = (long long)l;  // the same float -> int64 conversion as the kernel's
+      lvl = (L64 >= 0 && L64 < n_levels) ? (int)L64 : -1;
+    }
+    float* out = want.data() + n * C * PS * PS;
+    if (lvl < 0) {
+      std::fill(out, out + C * PS * PS, 0.f);
+      continue;
+    }
+    const LevelDesc& lv = p.lv[lvl];
+    const float ml = (float)std::min(lv.h - 1, lv.w - 1), wf = (float)(lv.w - 1), hf = (float)(lv.h - 1);
+    const float t00 = ml * a, t01 = ml * b, t02 = wf * x, t10 = ml * c, t11 = ml * d, t12 = hf * y, iw = 1.0f / wf, ih = 1.0f / hf;
+    for (int i = 0; i < PS; ++i)
+      for (int j = 0; j < PS; ++j) {
+        const float gx = ((2.0f * (fmaf(base[i], t01, base[j] * t00) + t02)) * iw) - 1.0f;
+        const float gy = ((2.0f * (fmaf(base[i], t11, base[j] * t10) + t12)) * ih) - 1.0f;
+        for (int ch = 0; ch < C; ++ch)
+          out[(size_t)ch * PS * PS + i * PS + j] = bilinear_border(lv.p + (n / N) * lv.sB + ch * lv.sC, lv.h, lv.w, lv.sH, gx, gy);
+      }
+  }
+  const std::string what = "laf_patches_kernel B=" + std::to_string(B) + " N=" + std::to_string(N) + " C=" + std::to_string(C) + " " +
+                           std::to_string(h) + "x" + std::to_string(w) + " PS=" + std::to_string(PS) + " levels=" + std::to_string(n_levels) +
+                           (normalize ? " norm" : " raw") + (select ? " pyramid" : " simple") + (row_pad ? " strided" : "") +
+                           (nonfinite ? " non-finite" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what, got.data(), want.data(), total);
+}
+
+// The fixed list (run_emu --patches): unbuilt levels (fewer levels than the clamp allows), non-finite LAFs, C = 3, PS = 1 and
+// 64, odd level sizes, a strided level 0, both functions and normalisations, grids that do not divide the patch count.
+static void test_patches_all() {
+  test_patches(1, 13, 1, 100, 120, 32, 2, true, true, 0, false, 3);
+  test_patches(2, 7, 3, 97, 131, 19, 3, true, true, 0, false, 4);
+  test_patches(2, 9, 3, 97, 131, 19, 3, false, true, 5, true, 5);
+  test_patches(1, 11, 1, 130, 167, 41, 2, true, true, 0, true, 2);
+  test_patches(1, 6, 2, 61, 53, 1, 5, true, true, 9, false, 3);
+  test_patches(1, 5, 1, 200, 150, 64, 2, true, true, 0, false, 2);
+  test_patches(2, 8, 3, 100, 120, 32, 1, true, false, 4, true, 3);
+  test_patches(1, 6, 1, 15, 23, 19, 1, false, true, 0, false, 1);
+}
+
 // The fixed lists (run_emu --sift / --orient): every configuration of the reference's tests and the envelope's edges, odd
 // batch sizes, grids that do not divide N, batch and row strides that are not P * P and P, special texels.
 static void test_sift_all() {
@@ -1968,6 +2082,11 @@ int main(int argc, char** argv) {
     }
     printf("%s: %d failing comparisons (per-patch gradient histograms, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures,
            emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--patches") {
+    test_patches_all();
+    printf("%s: %d failing comparisons (LAF patch extraction, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {
