@@ -335,6 +335,28 @@ int kb200_extract_patches_forward(const void* const* levels, const long long* le
                                   void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Affine shape (feature/affine_shape.py) in ONE kernel per call, one CTA per keypoint: the Baumberg second-moment matrix of
+ * the weighted Sobel gradients, summed in fp64, with the reference's degenerate-shape test and max normalisation.
+ * kb200_patch_affine_shape_forward (PatchAffineShapeEstimator):
+ *   x          fp32 (N, 1, P, P) patches with column stride 1 (batch and row element strides sB, sH); P <= 64
+ *   weighting  contiguous fp32 P x P
+ *   out        contiguous fp32 (N, 3): (a, b, c) / max(a, b, c)
+ * kb200_laf_affine_shape_forward (LAFAffineShapeEstimator with its default PatchAffineShapeEstimator):
+ *   levels, level_dims, n_levels, base   as for kb200_extract_patches_forward: the levels of (B_l, 1, h_l, w_l) images
+ *   laf        contiguous fp32 (B, N, 2, 3); B <= every level's batch
+ *   weighting  contiguous fp32 PS x PS; PS <= 64
+ *   out        contiguous fp32 (B, N, 2, 3): make_upright, the patch sampled at its level straight into shared memory
+ *              (no patch stack), the moments, ellipse_to_laf (closed-form inverse), the rescale to the input's scale and,
+ *              with preserve_orientation, the input's orientation; the centre copied.
+ * N = 0 (B * N = 0) launches nothing.  Forward only.
+ * ------------------------------------------------------------------------------------------ */
+int kb200_patch_affine_shape_forward(const void* x, const void* weighting, void* out, long long N, int P, long long sB, long long sH, float eps,
+                                     int dtype, void* stream);
+int kb200_laf_affine_shape_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                                   const void* weighting, void* out, long long B, long long N, int PS, float eps, int preserve_orientation,
+                                   int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Diagnostics (used by tests/): counts elements where the shared-reciprocal division of the tiled
  * warp kernel differs from IEEE division in a way that could change a sampled pixel.  `count`
  * (device int, zeroed by the caller) is incremented atomically.

@@ -31,9 +31,14 @@ def install(kornia_module=None) -> None:
     ``PatchDominantGradientOrientation``, which ``SIFTFeature``, ``SIFTFeatureScaleSpace`` and the ``LAFOrienter``
     constructor build by name, and the patch extraction ``extract_patches_from_pyramid`` / ``extract_patches_simple``
     that ``get_laf_descriptors`` / ``LAFDescriptor``, ``LAFOrienter`` and the affine shape estimators call by name (so
-    those reach the fused extraction at call time, whenever they were built).  Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``,
-    ``MultiResolutionDetector``, ``SIFTFeature``, ``SIFTFeatureScaleSpace`` or ``LAFOrienter`` built before ``install()``
-    keeps the reference pyramid, ``NonMaximaSuppression2d``, sub-pixel refiner, descriptor and orienter it holds.
+    those reach the fused extraction at call time, whenever they were built), and the affine shape estimators
+    ``PatchAffineShapeEstimator`` / ``LAFAffineShapeEstimator`` (classes).  A ``LAFAffineShapeEstimator`` built after
+    ``install()`` runs as one kernel per inference call; the reference's own ``LAFAffineShapeEstimator``, built before,
+    still builds its default ``PatchAffineShapeEstimator`` by name, so one constructed after ``install()`` gets the fused
+    patch estimator.  Rebinding a class affects modules constructed afterwards: a ``ScaleSpaceDetector``,
+    ``MultiResolutionDetector``, ``SIFTFeature``, ``SIFTFeatureScaleSpace``, ``LAFOrienter`` or ``LAFAffineShapeEstimator``
+    built before ``install()`` keeps the reference pyramid, ``NonMaximaSuppression2d``, sub-pixel refiner, descriptor,
+    orienter and affine shape estimator it holds.
 
     Every module of the package that holds a reference to one of the originals is patched: the
     defining modules and re-export sites (geometry/transform/__init__.py:30, geometry/__init__.py:40,
@@ -91,6 +96,10 @@ def install(kornia_module=None) -> None:
         # (affine_shape.py) import these by name and call them at call time
         "extract_patches_from_pyramid": ("feature.laf", feature.extract_patches_from_pyramid),
         "extract_patches_simple": ("feature.laf", feature.extract_patches_simple),
+        # classes: ScaleSpaceDetector(..., aff_module=LAFAffineShapeEstimator(...)) builds its estimator from this name, and
+        # LAFAffineShapeEstimator builds its default PatchAffineShapeEstimator from that name at construction
+        "PatchAffineShapeEstimator": ("feature.affine_shape", feature.PatchAffineShapeEstimator),
+        "LAFAffineShapeEstimator": ("feature.affine_shape", feature.LAFAffineShapeEstimator),
     }
     originals = {}
     for name, (mod, fn) in defining.items():

@@ -62,6 +62,9 @@ SIGNATURES = {
     "kb200_sift_describe_forward": (_i, [_vp] * 4 + [ctypes.c_longlong, _i, ctypes.c_longlong, ctypes.c_longlong] + [_i] * 6 + [ctypes.c_float] * 2 + [_i, _vp]),
     "kb200_patch_orientation_forward": (_i, [_vp] * 4 + [ctypes.c_longlong, _i, ctypes.c_longlong, ctypes.c_longlong, _i, ctypes.c_float, _i, _vp]),
     "kb200_extract_patches_forward": (_i, [_vp, _vp, _i, _vp, _vp, _vp, ctypes.c_longlong, ctypes.c_longlong] + [_i] * 5 + [_vp]),
+    "kb200_patch_affine_shape_forward": (_i, [_vp] * 3 + [ctypes.c_longlong, _i, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_float, _i, _vp]),
+    "kb200_laf_affine_shape_forward": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, ctypes.c_longlong, ctypes.c_longlong, _i, ctypes.c_float, _i, _i,
+                                            _vp]),
     "kb200_sepfilter_lerp_forward": (_i, [_vp] * 4 + [_i] * 10 + [ctypes.c_double, _i, _vp]),
     "kb200_debug_fastdiv_mismatches": (_i, [_vp, _vp, _i, _vp, _vp]),
 }

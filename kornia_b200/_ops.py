@@ -1021,6 +1021,65 @@ _define("extract_patches_fwd", "(Tensor[] levels, Tensor laf, int PS, bool norma
         first_tensor="the LAFs")
 
 
+def _patch_affine_shape_cuda(x, weighting, eps):
+    """(N, 1, 3) normalised second-moment shapes (a, b, c) of the (N, 1, P, P) patches ``x``."""
+    _require_cuda(x, "input")
+    _check_patch_args(x, weighting, "weighting")
+    N, P = x.shape[0], x.shape[-1]
+    out = torch.empty((N, 1, 3), device=x.device, dtype=x.dtype)
+    if N == 0:
+        return out
+    xs, wc = _patches(x), weighting.contiguous()
+    with torch.cuda.device(x.device), _Timed("patch_affine_shape_forward", x):
+        _lib.call("kb200_patch_affine_shape_forward", _ptr(xs), _ptr(wc), _ptr(out), N, P, xs.stride(0), xs.stride(-2), eps, _dtype_code(x),
+                  _stream(x))
+    _bump()
+    return out
+
+
+_define("patch_affine_shape_fwd", "(Tensor x, Tensor weighting, float eps) -> Tensor", _patch_affine_shape_cuda,
+        lambda x, weighting, eps: (_check_patch_args(x, weighting, "weighting"), x.new_empty((x.shape[0], 1, 3)))[1])
+
+
+def _check_laf_affine_args(levels, laf, weighting, PS: int) -> None:
+    """The patch extraction's levels and LAFs (one channel), and a PS x PS weighting of their dtype and device."""
+    _check_patch_levels(levels, laf, PS, True)
+    if levels[0].shape[1] != 1:
+        raise RuntimeError(f"kornia_b200: the affine shape is estimated on one-channel images, got {levels[0].shape[1]} channels")
+    if weighting.numel() != PS * PS or weighting.shape[-2:] != (PS, PS):
+        raise RuntimeError(f"kornia_b200: weighting must be {PS} x {PS}, got {tuple(weighting.shape)}")
+    _fake_same_device(laf, weighting)
+    _same(laf, weighting, "weighting")
+
+
+def _laf_affine_shape_cuda(levels, laf, weighting, PS, eps, preserve_orientation):
+    """(B, N, 2, 3) LAFs of ``laf`` with the affine shape estimated on ``levels`` (the image, then its pyrdowns)."""
+    _require_cuda(laf, "the LAFs")
+    _check_laf_affine_args(levels, laf, weighting, PS)
+    B, N = laf.shape[0], laf.shape[1]
+    out = torch.empty((B, N, 2, 3), device=laf.device, dtype=laf.dtype)
+    if B * N == 0:
+        return out
+    lv = [x if x.shape[-1] == 1 or x.stride(-1) == 1 else x.contiguous() for x in levels]
+    lafc, wc = laf.contiguous(), weighting.contiguous()
+    base = _affine_base(PS, laf.device)
+    ptrs = (ctypes.c_void_p * len(lv))(*[x.data_ptr() for x in lv])
+    dims = (ctypes.c_longlong * (5 * len(lv)))(*[v for x in lv for v in (x.shape[2], x.shape[3], x.stride(0), x.stride(1),
+                                                                         x.stride(2) if x.shape[2] > 1 else x.shape[3])])
+    with torch.cuda.device(laf.device), _Timed("laf_affine_shape_forward", laf):
+        _lib.call("kb200_laf_affine_shape_forward", ptrs, dims, len(lv), _ptr(lafc), _ptr(base), _ptr(wc), _ptr(out), B, N, PS, eps,
+                  int(preserve_orientation), _dtype_code(laf), _stream(laf))
+    _bump()
+    return out
+
+
+_define("laf_affine_shape_fwd", "(Tensor[] levels, Tensor laf, Tensor weighting, int PS, float eps, bool preserve_orientation) -> Tensor",
+        _laf_affine_shape_cuda,
+        lambda levels, laf, weighting, PS, eps, preserve_orientation: (_check_laf_affine_args(levels, laf, weighting, PS),
+                                                                        laf.new_empty((laf.shape[0], laf.shape[1], 2, 3)))[1],
+        first_tensor="the LAFs")
+
+
 def _sepfilter_lerp_cuda(x, kx, ky, border, weight):
     _require_cuda(x, "input")
     xc, kxc, kyc = x.contiguous(), kx.contiguous(), ky.contiguous()
@@ -1199,5 +1258,5 @@ OPERATORS: Tuple[str, ...] = (
     "filter2d_bwd_kernel", "sepfilter_fwd", "spatial_gradient_fwd", "spatial_gradient_bwd", "ssim_fwd", "sepfilter_lerp_fwd", "pyrdown_fwd",
     "undistort_fwd", "warp_u8hwc_fwd", "undistort_u8hwc_fwd", "rotation_matrix2d", "perspective_from_points", "feature_response_fwd",
     "scale_octave_fwd", "nms2d_fwd", "nms3d_fwd", "nms3d_minmax_fwd", "quad_interp3d_fwd", "sift_describe_fwd",
-    "patch_orientation_fwd", "extract_patches_fwd",
+    "patch_orientation_fwd", "extract_patches_fwd", "patch_affine_shape_fwd", "laf_affine_shape_fwd",
 )

@@ -726,6 +726,45 @@ int kb200_extract_patches_forward(const void* const* levels, const long long* le
   return extract_patches_forward(levels, level_dims, n_levels, laf, base, out, B, N, C, PS, normalize, select_level, (cudaStream_t)stream);
 }
 
+namespace kb200 {
+// affine_shape.cu (its kernels are not templates, so its header is included there only)
+int patch_affine_shape_forward(const float* x, const float* weighting, float* out, long long N, int P, long long sB, long long sH, float eps,
+                               cudaStream_t st);
+int laf_affine_shape_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                             const void* weighting, void* out, long long B, long long N, int PS, float eps, int preserve_orientation,
+                             cudaStream_t st);
+}  // namespace kb200
+
+int kb200_patch_affine_shape_forward(const void* x, const void* weighting, void* out, long long N, int P, long long sB, long long sH, float eps,
+                                     int dtype, void* stream) {
+  KB_CHECK_ARG(N >= 0 && P > 0, "bad sizes N=%lld P=%d", N, P);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused affine shape estimate is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  if (N == 0) return KB200_OK;
+  KB_CHECK_ARG(x && weighting && out, "null pointer argument");
+  const int rc = patch_affine_shape_forward((const float*)x, (const float*)weighting, (float*)out, N, P, sB, sH, eps, (cudaStream_t)stream);
+  if (rc == KB200_EUNSUPPORTED) set_error("patch size %d is outside the fused affine shape kernel's envelope", P);
+  return rc;
+}
+
+int kb200_laf_affine_shape_forward(const void* const* levels, const long long* level_dims, int n_levels, const void* laf, const void* base,
+                                   const void* weighting, void* out, long long B, long long N, int PS, float eps, int preserve_orientation,
+                                   int dtype, void* stream) {
+  KB_CHECK_ARG(B >= 0 && N >= 0 && PS > 0, "bad sizes B=%lld N=%lld PS=%d", B, N, PS);
+  KB_CHECK_ARG(dtype == KB200_F32 || dtype == KB200_F64, "bad dtype %d", dtype);
+  if (dtype != KB200_F32) {
+    set_error("the fused LAF affine shape estimate is fp32 only");
+    return KB200_EUNSUPPORTED;
+  }
+  const int rc = laf_affine_shape_forward(levels, level_dims, n_levels, laf, base, weighting, out, B, N, PS, eps, preserve_orientation,
+                                          (cudaStream_t)stream);
+  if (rc == KB200_EUNSUPPORTED) set_error("patch size %d is outside the fused affine shape kernel's envelope", PS);
+  return rc;
+}
+
 int kb200_sepfilter_lerp_forward(const void* x, const void* kernel_x, const void* kernel_y, void* out, int B, int C, int H, int W,
                                  int Bkx, int kw, int Bky, int kh, int border, int same, double weight, int dtype, void* stream) {
   int rc = check_filter(x, kernel_x, B, C, H, W, Bkx, kh, kw, border, same, dtype);

@@ -15,19 +15,11 @@
 //   sample = PixelSampler<float, BILINEAR, BORDER> at unnormalize(gx, w_l), unnormalize(gy, h_l), align_corners=False
 // bx, by come from the cached base vector (linspace(-1, 1, PS) * (PS - 1) / PS, built with torch ops on the device).
 #pragma once
-#include "sampler.cuh"
+#include "laf_map.cuh"
 
 namespace kb200 {
 
 constexpr int LP_NT = 128;          // threads per CTA: 19 x 19 = 361 pixels are 3 rounds of 128 (94 % of the lanes busy)
-constexpr int LP_MAX_LEVELS = 32;
-
-// A level the kernel samples: (B_l, C, h, w) fp32 with column stride 1.
-struct LevelDesc {
-  const float* p;
-  long long sB, sC;
-  int h, w, sH;
-};
 
 struct LafPatchParams {
   LevelDesc lv[LP_MAX_LEVELS];
@@ -41,54 +33,9 @@ struct LafPatchParams {
   float max_clamp;          // max(0, min(h, w) // PS - 1)
 };
 
-// ATen's .long() of a NaN level on the device: the same conversion instruction ATen's CUDA copy kernel issues.
-__device__ __forceinline__ long long level_of(float l) { return (long long)l; }
-
-// The per-patch scalars: the chosen level (-1 when it is not one of the n_levels sampled) and the level's affine map.
-struct PatchMap {
-  int level;
-  float t00, t01, t02, t10, t11, t12;
-  float inv_w, inv_h;  // fp32 1 / (w_l - 1), 1 / (h_l - 1)
-};
-
 __device__ __forceinline__ PatchMap laf_patch_map(const LafPatchParams& p, long long n) {
-  using R = RN<float>;
   const float* L = p.laf + n * 6;
-  float a = ldg(L + 0), b = ldg(L + 1), x = ldg(L + 2), c = ldg(L + 3), d = ldg(L + 4), y = ldg(L + 5);
-  if (p.normalize) {
-    a = R::mul(p.n_lin, a); b = R::mul(p.n_lin, b); x = R::mul(p.n_tx, x);
-    c = R::mul(p.n_lin, c); d = R::mul(p.n_lin, d); y = R::mul(p.n_ty, y);
-  }
-  PatchMap m;
-  int lvl = 0;
-  if (p.select_level) {
-    const float m0 = (float)min(p.lv[0].h - 1, p.lv[0].w - 1);
-    const float da = R::mul(m0, a), db = R::mul(m0, b), dc = R::mul(m0, c), dd = R::mul(m0, d);
-    const float det = R::add(R::sub(R::mul(da, dd), R::mul(dc, db)), 1e-10f);
-    const float s = R::mul(R::mul(2.0f, __fsqrt_rn(fabsf(det))), R::div(1.0f, (float)p.PS));
-    float l = log2f(s);
-    if (!(l != l)) l = fminf(fmaxf(l, 0.0f), p.max_clamp);
-    const long long L64 = level_of(l);
-    lvl = (L64 >= 0 && L64 < p.n_levels) ? (int)L64 : -1;
-  }
-  m.level = lvl;
-  if (lvl < 0) return m;
-  const int h = p.lv[lvl].h, w = p.lv[lvl].w;
-  const float ml = (float)min(h - 1, w - 1), wf = (float)(w - 1), hf = (float)(h - 1);
-  m.t00 = R::mul(ml, a); m.t01 = R::mul(ml, b); m.t02 = R::mul(wf, x);
-  m.t10 = R::mul(ml, c); m.t11 = R::mul(ml, d); m.t12 = R::mul(hf, y);
-  m.inv_w = R::div(1.0f, wf);
-  m.inv_h = R::div(1.0f, hf);
-  return m;
-}
-
-// The normalised sampling coordinate of base point (bx, by) (grid_sample's input, before unnormalize).
-__device__ __forceinline__ void laf_grid_point(const PatchMap& m, float bx, float by, float& gx, float& gy) {
-  using R = RN<float>;
-  gx = R::add(R::fma(by, m.t01, R::mul(bx, m.t00)), m.t02);
-  gy = R::add(R::fma(by, m.t11, R::mul(bx, m.t10)), m.t12);
-  gx = R::sub(R::mul(R::mul(2.0f, gx), m.inv_w), 1.0f);
-  gy = R::sub(R::mul(R::mul(2.0f, gy), m.inv_h), 1.0f);
+  return laf_patch_map(p, ldg(L + 0), ldg(L + 1), ldg(L + 2), ldg(L + 3), ldg(L + 4), ldg(L + 5));
 }
 
 __global__ void __launch_bounds__(LP_NT, 8) laf_patches_kernel(const __grid_constant__ LafPatchParams p) {

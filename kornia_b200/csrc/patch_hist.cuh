@@ -1,5 +1,6 @@
 // kornia_b200 -- device code shared by the per-patch gradient-histogram kernels: SIFTDescriptor.forward (siftdesc.cuh)
-// and PatchDominantGradientOrientation.forward (patch_orientation.cuh).
+// and PatchDominantGradientOrientation.forward (patch_orientation.cuh); the staging, gradient and block sum also serve the
+// second-moment kernels of affine_shape.cuh.
 //
 // One CTA owns one patch at a time (persistent CTAs stride over the N patches), so a patch's result is a pure function of
 // the patch: every sum runs in an order fixed by the thread layout, with no atomics and nothing depending on the grid or on
@@ -47,13 +48,10 @@ __device__ __forceinline__ void ph_stage(const float* __restrict__ src, long lon
   }
 }
 
-// Pixel e of the staged patch: its first bin (-1 when the angle is NaN) and the weights of its two bins.
-//   mag = sqrt(gx * gx + gy * gy + eps) * weight;  ori = atan2(gy, gx + eps) + 2 pi;  o = A * (ori [+ pi]) / (2 pi)
-template <bool ADD_PI>
-__device__ __forceinline__ void ph_bin_pixel(const float* s_patch, int P, int e, const GradStencil& st, float eps, float weight, int A,
-                                             int& b0, float& w0, float& w1) {
+// The gradient (g[0] = d/dx, g[1] = d/dy) of pixel e of the staged patch.
+__device__ __forceinline__ void ph_gradient(const float* s_patch, int P, int e, const GradStencil& st, float g[2]) {
   const int y = e / P, x = e - y * P;
-  float g[2] = {0.f, 0.f};
+  g[0] = g[1] = 0.f;
 #pragma unroll
   for (int r = 0; r < 3; ++r) {
     const int yy = min(max(y + r - 1, 0), P - 1);
@@ -64,6 +62,15 @@ __device__ __forceinline__ void ph_bin_pixel(const float* s_patch, int P, int e,
       for (int o = 0; o < 2; ++o) g[o] = __fmaf_rn(st.t[o][r][c], v, g[o]);
     }
   }
+}
+
+// Pixel e of the staged patch: its first bin (-1 when the angle is NaN) and the weights of its two bins.
+//   mag = sqrt(gx * gx + gy * gy + eps) * weight;  ori = atan2(gy, gx + eps) + 2 pi;  o = A * (ori [+ pi]) / (2 pi)
+template <bool ADD_PI>
+__device__ __forceinline__ void ph_bin_pixel(const float* s_patch, int P, int e, const GradStencil& st, float eps, float weight, int A,
+                                             int& b0, float& w0, float& w1) {
+  float g[2];
+  ph_gradient(s_patch, P, e, st, g);
   const float gx = g[0], gy = g[1];
   float mag = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), eps));
   const float ori = __fadd_rn(atan2f(gy, __fadd_rn(gx, eps)), PH_TWO_PI);

@@ -1,5 +1,7 @@
 """Drop-in ``extract_patches_from_pyramid`` and ``extract_patches_simple``, with the helpers their composition needs:
-``get_laf_scale``, ``normalize_laf``, ``denormalize_laf`` and ``generate_patch_grid_from_normalized_LAF`` (reference:
+``get_laf_scale``, ``normalize_laf``, ``denormalize_laf`` and ``generate_patch_grid_from_normalized_LAF``, and the LAF helpers
+of the affine shape estimators (feature/affine_shape.py): ``make_upright``, ``scale_laf``, ``ellipse_to_laf``,
+``get_laf_orientation``, ``set_laf_orientation`` and ``rotate_laf``, each the reference's op sequence (reference:
 kornia/feature/laf.py).
 
 The reference cuts patches out of a pyramid by looping over every level the image allows and, inside that, over every
@@ -17,15 +19,19 @@ Every other call runs ``_composed_extract_pyramid`` / ``_composed_extract_simple
 ``F.affine_grid``, ``F.grid_sample`` and this library's ``pyrdown``, which is also the differentiable path."""
 from __future__ import annotations
 
+from typing import Union
+
 import torch
 import torch.nn.functional as F
 
 from .. import _ops
 from ..core.check import check_shape
+from ..geometry.transform.matrices import angle_to_rotation_matrix, rad2deg
 from ..geometry.transform.pyramid import pyrdown
 
 __all__ = ["extract_patches_from_pyramid", "extract_patches_simple", "get_laf_scale", "normalize_laf", "denormalize_laf",
-           "generate_patch_grid_from_normalized_LAF"]
+           "generate_patch_grid_from_normalized_LAF", "get_laf_orientation", "rotate_laf", "set_laf_orientation", "scale_laf", "make_upright",
+           "ellipse_to_laf"]
 
 def _check_laf(laf: torch.Tensor) -> None:
     """KORNIA_CHECK_LAF: a (B, N, 2, 3) tensor."""
@@ -38,6 +44,65 @@ def get_laf_scale(LAF: torch.Tensor) -> torch.Tensor:
     eps = 1e-10
     out = LAF[..., 0:1, 0:1] * LAF[..., 1:2, 1:2] - LAF[..., 1:2, 0:1] * LAF[..., 0:1, 1:2] + eps
     return out.abs().sqrt()
+
+
+def get_laf_orientation(LAF: torch.Tensor) -> torch.Tensor:
+    """(B, N, 1) orientation of the LAFs in degrees: rad2deg(atan2(LAF[..., 0, 1], LAF[..., 0, 0]))."""
+    _check_laf(LAF)
+    angle_rad = torch.atan2(LAF[..., 0, 1], LAF[..., 0, 0])
+    return rad2deg(angle_rad).unsqueeze(-1)
+
+
+def rotate_laf(LAF: torch.Tensor, angles_degrees: torch.Tensor) -> torch.Tensor:
+    """The LAFs with their linear part multiplied on the right by the rotation of ``angles_degrees`` (B, N, 1)."""
+    _check_laf(LAF)
+    B, N = LAF.shape[:2]
+    rotmat = angle_to_rotation_matrix(angles_degrees).view(B * N, 2, 2)
+    out_laf = LAF.clone()
+    out_laf[:, :, :2, :2] = torch.bmm(LAF[:, :, :2, :2].reshape(B * N, 2, 2), rotmat).reshape(B, N, 2, 2)
+    return out_laf
+
+
+def set_laf_orientation(LAF: torch.Tensor, angles_degrees: torch.Tensor) -> torch.Tensor:
+    """The LAFs rotated so that their orientation becomes ``angles_degrees`` (B, N, 1)."""
+    _check_laf(LAF)
+    ori = get_laf_orientation(LAF).reshape_as(angles_degrees)
+    return rotate_laf(LAF, angles_degrees - ori)
+
+
+def scale_laf(laf: torch.Tensor, scale_coef: Union[float, torch.Tensor]) -> torch.Tensor:
+    """The LAFs with their linear part multiplied by ``scale_coef`` (a float or a broadcastable tensor); centres kept."""
+    if not isinstance(scale_coef, (float, torch.Tensor)):
+        raise TypeError(f"scale_coef should be float or torch.Tensor. Got {type(scale_coef)}")
+    _check_laf(laf)
+    centerless_laf = laf[:, :, :2, :2]
+    return torch.cat([scale_coef * centerless_laf, laf[:, :, :, 2:]], dim=3)
+
+
+def make_upright(laf: torch.Tensor, eps: float = 1e-9) -> torch.Tensor:
+    """The LAFs with their rotation removed (the U * S of a 2 x 2 SVD U S V^T), scale and centre kept."""
+    _check_laf(laf)
+    det = get_laf_scale(laf)
+    scale = det
+    b2a2 = torch.sqrt(laf[..., 0:1, 1:2] ** 2 + laf[..., 0:1, 0:1] ** 2) + eps
+    laf1_ell = torch.cat([(b2a2 / det).contiguous(), torch.zeros_like(det)], dim=3)
+    laf2_ell = torch.cat([((laf[..., 1:2, 1:2] * laf[..., 0:1, 1:2] + laf[..., 1:2, 0:1] * laf[..., 0:1, 0:1]) / (b2a2 * det)),
+                          (det / b2a2).contiguous()], dim=3)
+    laf_unit_scale = torch.cat([torch.cat([laf1_ell, laf2_ell], dim=2), laf[..., :, 2:3]], dim=3)
+    return scale_laf(laf_unit_scale, scale)
+
+
+def ellipse_to_laf(ells: torch.Tensor) -> torch.Tensor:
+    """(B, N, 2, 3) LAFs of (B, N, 5) ellipses [x, y, a, b, c]: the inverse of the lower-triangular square root
+    [[sqrt|a|, 0], [b / (sqrt|a| + sqrt|c|), sqrt|c|]] of [[a, b], [b, c]], centred at (x, y)."""
+    check_shape(ells, ["B", "N", "5"])
+    B, N, _ = ells.shape
+    a11 = ells[..., 2:3].abs().sqrt()
+    a12 = torch.zeros_like(a11)
+    a22 = ells[..., 4:5].abs().sqrt()
+    a21 = ells[..., 3:4] / (a11 + a22).clamp(1e-9)
+    A = torch.stack([a11, a12, a21, a22], dim=-1).view(B, N, 2, 2).inverse()
+    return torch.cat([A, ells[..., :2].view(B, N, 2, 1)], dim=3)
 
 
 def denormalize_laf(LAF: torch.Tensor, images: torch.Tensor) -> torch.Tensor:

@@ -19,6 +19,12 @@ def deg2rad(tensor: torch.Tensor) -> torch.Tensor:
     return tensor * _PI.to(tensor.device).type(tensor.dtype) / 180.0
 
 
+def rad2deg(tensor: torch.Tensor) -> torch.Tensor:
+    if not isinstance(tensor, torch.Tensor):
+        raise TypeError(f"Input type is not a torch.Tensor. Got {type(tensor)}")
+    return 180.0 * tensor / _PI.to(tensor.device).type(tensor.dtype)
+
+
 def angle_to_rotation_matrix(angle: torch.Tensor) -> torch.Tensor:
     """(*,) degrees -> (*,2,2) [[cos, sin], [-sin, cos]]."""
     rad = deg2rad(angle)

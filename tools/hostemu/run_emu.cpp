@@ -21,6 +21,7 @@
 #include "../../kornia_b200/csrc/siftdesc.cuh"
 #include "../../kornia_b200/csrc/patch_orientation.cuh"
 #include "../../kornia_b200/csrc/laf_patches.cuh"
+#include "../../kornia_b200/csrc/affine_shape.cuh"
 #include "../../kornia_b200/csrc/remap_tiled.cuh"
 #include "ref_ssim_tiled.cuh"
 #include "../../kornia_b200/csrc/warp_bwd_tma2.cuh"
@@ -45,6 +46,8 @@ alignas(128) unsigned char bwd2_smem[256 * 1024];
 alignas(128) unsigned char u8t_smem[256 * 1024];
 alignas(128) unsigned char sift_smem[128 * 1024];
 alignas(128) unsigned char ori_smem[128 * 1024];
+alignas(128) unsigned char paff_smem[64 * 1024];
+alignas(128) unsigned char laff_smem[64 * 1024];
 void set_error(const char*, ...) {}
 }  // namespace kb200
 
@@ -1133,6 +1136,176 @@ static void test_patches_all() {
   test_patches(1, 6, 1, 15, 23, 19, 1, false, true, 0, false, 1);
 }
 
+// Scalar restatement of PatchAffineShapeEstimator.forward / LAFAffineShapeEstimator.forward (kornia/feature/affine_shape.py)
+// in the kernels' op order (csrc/affine_shape.cuh): the weighted Sobel products summed in fp64 per thread (pixels e = t,
+// t + 256, ...) then per warp in order, one rounding of sum / P^2; the degenerate mask and max normalisation; for LAFs
+// make_upright, the level and map of test_patches, ATen's bilinear 'border' sampling, ellipse_to_laf's closed-form inverse,
+// the rescale and the orientation restore.  NaN matches NaN.
+static void aff_moments_ref(const float* patch, int P, const float* wt, float m[3]) {
+  const GradStencil st = sobel_stencil();
+  std::vector<double> part[3];
+  for (int k = 0; k < 3; ++k) part[k].assign(PH_NT, 0.0);
+  for (int e = 0; e < P * P; ++e) {
+    const int y = e / P, x = e % P;
+    float g[2] = {0.f, 0.f};
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        const float v = patch[std::min(std::max(y + r - 1, 0), P - 1) * P + std::min(std::max(x + c - 1, 0), P - 1)];
+        for (int o = 0; o < 2; ++o) g[o] = fmaf(st.t[o][r][c], v, g[o]);
+      }
+    const float gx = g[0] * wt[e], gy = g[1] * wt[e];
+    part[0][e % PH_NT] += (double)(gx * gx);
+    part[1][e % PH_NT] += (double)(gx * gy);
+    part[2][e % PH_NT] += (double)(gy * gy);
+  }
+  for (int k = 0; k < 3; ++k) m[k] = (float)(block_sum(part[k]) / (double)(P * P));
+}
+static void aff_tail_ref(float m[3], float eps) {
+  const int nb = (m[0] < eps) + (m[1] < eps) + (m[2] < eps);
+  const float bad = nb >= 2 ? 1.f : 0.f, keep = 1.f - bad, circ[3] = {1.f, 0.f, 1.f};
+  for (int k = 0; k < 3; ++k) m[k] = m[k] * keep + circ[k] * bad;
+  float mx = m[0];
+  for (int k = 1; k < 3; ++k)
+    if (m[k] > mx || m[k] != m[k]) mx = m[k];
+  for (int k = 0; k < 3; ++k) m[k] = m[k] / mx;
+}
+static float scale_ref(float a, float b, float c, float d) { return sqrtf(fabsf((a * d - c * b) + 1e-10f)); }
+
+// Patches: smooth, constant (degenerate), one-direction stripes, anti-correlated ramps (negative b) and special texels.
+static void test_patch_affine(long long N, int P, float eps, int specials, unsigned grid) {
+  const int sH = P + 2;
+  const long long sB = (long long)sH * P + 3;
+  std::vector<float> x = make_patches(N, P, sB, sH, specials), wt = randv(P * P, 0.1f, 1.f);
+  for (long long n = 0; n < N; ++n)
+    for (int y = 0; y < P; ++y)
+      for (int xx = 0; xx < P; ++xx) {
+        float& v = x[(size_t)(n * sB + y * sH + xx)];
+        if (n % 5 == 1) v = 0.25f;                          // constant
+        if (n % 5 == 2) v = (float)((xx / 3) % 2);          // vertical stripes: gy = 0
+        if (n % 5 == 3) v = 0.1f * (float)(xx - y) + 0.01f * v;  // anti-correlated gradients: b < 0
+      }
+  std::vector<float> got((size_t)(N * 3), -777.f), want((size_t)(N * 3));
+  PatchAffParams p{x.data(), wt.data(), got.data(), sB, sH, N, P, eps};
+  emu::launch(grid, dim3(PH_NT), [&] { patch_affine_shape_kernel(p); });
+  std::vector<float> patch(P * P);
+  for (long long n = 0; n < N; ++n) {
+    for (int y = 0; y < P; ++y)
+      for (int xx = 0; xx < P; ++xx) patch[y * P + xx] = x[(size_t)(n * sB + y * sH + xx)];
+    float m[3];
+    aff_moments_ref(patch.data(), P, wt.data(), m);
+    aff_tail_ref(m, eps);
+    for (int k = 0; k < 3; ++k) want[n * 3 + k] = m[k];
+  }
+  const std::string what = "patch_affine_shape_kernel N=" + std::to_string(N) + " P=" + std::to_string(P) + " eps=" + std::to_string(eps) +
+                           (specials ? " special texels" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what, got.data(), want.data(), got.size());
+}
+
+static void test_laf_affine(int B, long long N, int h, int w, int PS, int n_levels, bool preserve, bool nonfinite, int extra_images,
+                            unsigned grid) {
+  const int Bimg = B + extra_images;
+  std::vector<std::vector<float>> store(n_levels);
+  LafAffParams p{};
+  int hl = h, wl = w;
+  for (int l = 0; l < n_levels; ++l, hl /= 2, wl /= 2) {
+    const int sH = wl + (l == 0 ? 3 : 0);
+    const long long sB = (long long)sH * hl + (l == 0 ? 5 : 0);
+    store[l] = randv((size_t)(sB * Bimg), 0.f, 1.f);
+    for (long long i = 0; i < sB * Bimg; i += 7) store[l][i] *= 0.3f;  // texture
+    p.lv[l] = LevelDesc{store[l].data(), sB, sB, hl, wl, sH};
+  }
+  std::vector<float> laf((size_t)(B * N * 6)), base(PS), wt = randv(PS * PS, 0.1f, 1.f);
+  for (long long n = 0; n < B * N; ++n) {
+    const float u = randv(1, -1.5f, (float)n_levels + 1.5f)[0], s = powf(2.f, u) * PS / 2.f, a = randv(1, 0.f, 6.2831853f)[0];
+    const float sh = randv(1, -0.3f, 0.3f)[0], r = randv(1, 0.6f, 1.6f)[0];
+    float* L = laf.data() + n * 6;
+    L[0] = s * cosf(a) * r; L[1] = s * (cosf(a) * sh - sinf(a) / r); L[2] = randv(1, -0.2f, 1.2f)[0] * (w - 1);
+    L[3] = s * sinf(a) * r; L[4] = s * (sinf(a) * sh + cosf(a) / r); L[5] = randv(1, -0.2f, 1.2f)[0] * (h - 1);
+    if (nonfinite && n % 4 == 1) L[(n / 4) % 6] = (n % 8 == 1) ? NAN : ((n % 16 == 5) ? -INFINITY : INFINITY);
+  }
+  for (int j = 0; j < PS; ++j) base[j] = PS > 1 ? (-1.f + 2.f * j / (float)(PS - 1)) * (float)(PS - 1) / (float)PS : 0.f;
+  std::vector<float> got((size_t)(B * N * 6), -777.f), want((size_t)(B * N * 6));
+  p.laf = laf.data();
+  p.base = base.data();
+  p.weighting = wt.data();
+  p.out = got.data();
+  p.N = N;
+  p.total = B * N;
+  p.PS = PS;
+  p.n_levels = n_levels;
+  p.n_lin = 1.0f / (float)std::min(h - 1, w - 1);
+  p.n_tx = (float)(1.0 / (double)(w - 1));
+  p.n_ty = (float)(1.0 / (double)(h - 1));
+  p.max_clamp = (float)std::max(0, std::min(h, w) / PS - 1);
+  p.eps = 1e-10f;
+  p.preserve_orientation = preserve;
+  emu::launch(grid, dim3(PH_NT), [&] { laf_affine_shape_kernel(p); });
+  std::vector<float> patch(PS * PS);
+  for (long long n = 0; n < B * N; ++n) {
+    const float* L = laf.data() + n * 6;
+    const float a0 = L[0], b0 = L[1], c0 = L[3], d0 = L[4];
+    const float det = scale_ref(a0, b0, c0, d0), b2a2 = sqrtf(b0 * b0 + a0 * a0) + 1e-9f;
+    float a = det * (b2a2 / det), b = det * 0.f, x = L[2], c = det * ((d0 * b0 + c0 * a0) / (b2a2 * det)), d = det * (det / b2a2), y = L[5];
+    a = p.n_lin * a; b = p.n_lin * b; x = p.n_tx * x; c = p.n_lin * c; d = p.n_lin * d; y = p.n_ty * y;
+    const float m0 = (float)std::min(h - 1, w - 1);
+    const float sc = (2.0f * sqrtf(fabsf(((m0 * a) * (m0 * d) - (m0 * c) * (m0 * b)) + 1e-10f))) * (1.0f / (float)PS);
+    float l = log2f(sc);
+    if (l == l) l = std::fmin(std::fmax(l, 0.f), p.max_clamp);
+    const long long L64 = (long long)l;
+    const int lvl = (L64 >= 0 && L64 < n_levels) ? (int)L64 : -1;
+    float m[3] = {0.f, 0.f, 0.f};
+    if (lvl >= 0) {
+      const LevelDesc& lv = p.lv[lvl];
+      const float ml = (float)std::min(lv.h - 1, lv.w - 1), wf = (float)(lv.w - 1), hf = (float)(lv.h - 1);
+      const float t00 = ml * a, t01 = ml * b, t02 = wf * x, t10 = ml * c, t11 = ml * d, t12 = hf * y, iw = 1.0f / wf, ih = 1.0f / hf;
+      for (int i = 0; i < PS; ++i)
+        for (int j = 0; j < PS; ++j) {
+          const float gx = ((2.0f * (fmaf(base[i], t01, base[j] * t00) + t02)) * iw) - 1.0f;
+          const float gy = ((2.0f * (fmaf(base[i], t11, base[j] * t10) + t12)) * ih) - 1.0f;
+          patch[i * PS + j] = bilinear_border(lv.p + (n / N) * lv.sB, lv.h, lv.w, lv.sH, gx, gy);
+        }
+      aff_moments_ref(patch.data(), PS, wt.data(), m);
+    }
+    aff_tail_ref(m, p.eps);
+    const float a11 = sqrtf(fabsf(m[0])), a22 = sqrtf(fabsf(m[2]));
+    float den = a11 + a22;
+    if (den == den) den = std::fmax(den, 1e-9f);
+    const float a21 = m[1] / den, i00 = 1.f / a11, i11 = 1.f / a22, i10 = -(a21 / (a11 * a22)), i01 = 0.f;
+    const float coef = det / scale_ref(i00, i01, i10, i11);
+    float o[4] = {coef * i00, coef * i01, coef * i10, coef * i11};
+    if (preserve) {
+      const float pi = 3.14159274101257324219f;
+      const float ang = (180.f * atan2f(b0, a0)) / pi - (180.f * atan2f(o[1], o[0])) / pi;
+      const float rad = (ang * pi) * (1.f / 180.f), cs = cosf(rad), sn = sinf(rad);
+      const float r[2][2] = {{cs, sn}, {-sn, cs}}, lm[2][2] = {{o[0], o[1]}, {o[2], o[3]}};
+      for (int i = 0; i < 2; ++i)
+        for (int j = 0; j < 2; ++j) o[2 * i + j] = fmaf(lm[i][1], r[1][j], lm[i][0] * r[0][j]);
+    }
+    float* out = want.data() + n * 6;
+    out[0] = o[0]; out[1] = o[1]; out[2] = L[2]; out[3] = o[2]; out[4] = o[3]; out[5] = L[5];
+  }
+  const std::string what = "laf_affine_shape_kernel B=" + std::to_string(B) + " N=" + std::to_string(N) + " " + std::to_string(h) + "x" +
+                           std::to_string(w) + " PS=" + std::to_string(PS) + " levels=" + std::to_string(n_levels) +
+                           (preserve ? " preserve" : " upright") + (nonfinite ? " non-finite" : "") +
+                           (extra_images ? " extra images" : "") + " grid=" + std::to_string(grid);
+  compare_bits_or_nan(what, got.data(), want.data(), got.size());
+}
+
+// The fixed list (run_emu --affine): P = 19, 32, 41, 64 and 3; constant, stripe and negative-b patches, special texels, a
+// non-default eps; LAFs at unbuilt levels, non-finite LAFs, both preserve_orientation values, more images than LAF sets,
+// grids that do not divide the keypoint count.
+static void test_affine_all() {
+  test_patch_affine(11, 19, 1e-10f, 0, 3);
+  test_patch_affine(7, 32, 1e-10f, 1, 2);
+  test_patch_affine(6, 41, 1e-4f, 0, 4);
+  test_patch_affine(4, 64, 1e-10f, 1, 3);
+  test_patch_affine(5, 3, 1e-10f, 0, 2);
+  test_laf_affine(1, 13, 100, 120, 32, 2, true, false, 0, 3);
+  test_laf_affine(2, 9, 97, 131, 19, 3, false, true, 0, 4);
+  test_laf_affine(1, 11, 130, 167, 41, 2, true, true, 1, 2);
+  test_laf_affine(2, 7, 61, 53, 19, 1, true, false, 0, 5);
+}
+
 // The fixed lists (run_emu --sift / --orient): every configuration of the reference's tests and the envelope's edges, odd
 // batch sizes, grids that do not divide N, batch and row strides that are not P * P and P, special texels.
 static void test_sift_all() {
@@ -2087,6 +2260,11 @@ int main(int argc, char** argv) {
   if (argc == 2 && std::string(argv[1]) == "--patches") {
     test_patches_all();
     printf("%s: %d failing comparisons (LAF patch extraction, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
+    return failures ? 1 : 0;
+  }
+  if (argc == 2 && std::string(argv[1]) == "--affine") {
+    test_affine_all();
+    printf("%s: %d failing comparisons (affine shape, %d of them bit-level)\n", failures ? "FAILED" : "PASSED", failures, emu_strict_failures);
     return failures ? 1 : 0;
   }
   if (argc == 2 && std::string(argv[1]) == "--specials") {
